@@ -382,9 +382,9 @@ def eval_expr(e, table):
         return v, (np.ones(n, bool) if c.valid is None else c.valid)
     if op == "lit":
         val = e[1]
-        if val is None:
-            return np.zeros(n, np.int64), np.zeros(n, bool)
         dt = e[2] if len(e) > 2 else None
+        if val is None:                      # a typed NULL keeps its class
+            return np.zeros(n, dt or np.int64), np.zeros(n, bool)
         if dt is None:
             dt = np.float64 if isinstance(val, float) else (bool if isinstance(val, bool) else np.int64)
         return np.full(n, val, dtype=dt), np.ones(n, bool)
@@ -399,7 +399,7 @@ def eval_expr(e, table):
         a, av = eval_expr(e[1], table); b, bv = eval_expr(e[2], table)
         a = a.astype(np.float64); b = b.astype(np.float64)
         nz = b != 0
-        with np.errstate(divide="ignore", invalid="ignore"):
+        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
             r = np.where(nz, a / np.where(nz, b, 1.0), 0.0)
         return r, av & bv & nz
     if op == "neg":
@@ -440,10 +440,27 @@ def eval_expr(e, table):
     if op == "cast_f64":
         a, av = eval_expr(e[1], table)
         return a.astype(np.float64), av
-    if op == "cast_i64":
+    if op in ("cast_i64", "cast_i32"):
         a, av = eval_expr(e[1], table)
-        return a.astype(np.int64), av
+        dt = np.int64 if op == "cast_i64" else np.int32
+        if a.dtype.kind == "f":
+            return _java_double_to_int(a.astype(np.float64), dt), av
+        return a.astype(dt), av          # long -> int keeps the low 32 bits (JLS 5.1.3 narrowing)
     raise ValueError("unknown expression op %r" % (op,))
+
+
+def _java_double_to_int(a, dt):
+    """Java's (long) d / (int) d (JLS 5.1.3, what Cast.scala:1159-1161 `numeric.toLong` / `toInt` run): NaN -> 0, otherwise
+    rounded toward zero and saturated at the target's range.  numpy's astype would give INT64_MIN for NaN and +-inf."""
+    info = np.iinfo(dt)
+    hi = float(info.max) + 1.0                  # 2^31 / 2^63, exact in double
+    out = np.zeros(len(a), dt)
+    with np.errstate(invalid="ignore"):
+        big, small = a >= hi, a <= -hi
+        mid = ~(big | small | np.isnan(a))
+    out[big], out[small] = info.max, info.min
+    out[mid] = np.trunc(a[mid]).astype(dt)
+    return out
 
 
 def _col_from_eval(v, valid):

@@ -327,7 +327,7 @@ object ExprCompiler {
   def supported(e: Expression): Boolean = e match {
     case a: AttributeReference => GpuExec.typeId(a.dataType) > 0
     case Alias(c, _) => supported(c)
-    case l: Literal => l.value == null || vt(l.dataType) > 0
+    case l: Literal => vt(l.dataType) > 0        // a NULL literal too: LIT_NULL carries its class (an untyped NULL has none)
     case Add(l, r, _) => vt(e.dataType) > 1 && supported(l) && supported(r)
     case Subtract(l, r, _) => vt(e.dataType) > 1 && supported(l) && supported(r)
     case Multiply(l, r, _) => vt(e.dataType) > 1 && supported(l) && supported(r)
@@ -369,7 +369,7 @@ object ExprCompiler {
       case Not(c) => go(c); emit(32, 1)
       case IsNull(c) => go(c); emit(33, 1)
       case IsNotNull(c) => go(c); emit(34, 1)
-      case Cast(c, to, _, _) => go(c); emit(vt(to) match { case 4 => 40; case 3 => 41; case _ => 42 }, vt(to))
+      case Cast(c, to, _, _) => go(c); emit(vt(to) match { case 4 => 40; case 3 => 41; case _ => 42 }, vt(to), vt(c.dataType))   // arg = source class
       case other => throw new B200Exception(5, s"expression $other is not supported on the GPU path")
     }
     go(e)

@@ -64,8 +64,16 @@ void expr_validate(const sb_table *in, const sb_expr &e) {
   }
   if (has_decimal && e.n > 1 && !only_null_tests)
     fail(SB_ERR_UNSUPPORTED, "arithmetic / comparison on DECIMAL columns is not implemented on the GPU path (unscaled values would ignore the scale)");
+  // Type check: the kernels trust the vtypes (a CAST reads its source class from `arg`, a comparison compares as `arg`, arithmetic
+  // works at the node's vtype), so a program whose operands disagree with them would be evaluated on reinterpreted bits.  vt[] is
+  // the class of each stack slot; a NULL literal (null_lit[]) is accepted in any class.
+  int32_t vt[EXPR_STACK + 1];
+  bool null_lit[EXPR_STACK + 1];
+  int cols_seen[EXPR_MAX_COLS], ncols = 0;
+  auto operand_ok = [&](int slot, int32_t want) { return null_lit[slot] || vt[slot] == want; };
   for (int i = 0; i < e.n; i++) {
     const sb_expr_node &nd = e.nodes[i];
+    int32_t res = nd.vtype;
     switch (nd.op) {
       case SB_OP_COL: {
         SB_REQUIRE(nd.arg >= 0 && nd.arg < (int)in->cols.size(), "expression references column %d of %zu", nd.arg, in->cols.size());
@@ -75,23 +83,70 @@ void expr_validate(const sb_table *in, const sb_expr &e) {
         } else {
           SB_REQUIRE(nd.vtype == vtype_of_column(t), "COL node %d: vtype %d does not match column type %d", i, nd.vtype, t);
         }
-        depth++;
+        bool seen = false;
+        for (int c = 0; c < ncols; c++) seen |= cols_seen[c] == nd.arg;
+        if (!seen) {
+          SB_REQUIRE(ncols < EXPR_MAX_COLS, "expression references more than %d distinct columns", EXPR_MAX_COLS);
+          cols_seen[ncols++] = nd.arg;
+        }
         break;
       }
-      case SB_OP_LIT_I64: case SB_OP_LIT_F64: case SB_OP_LIT_NULL: depth++; break;
+      case SB_OP_LIT_I64:
+        SB_REQUIRE(nd.vtype >= SB_VT_BOOL && nd.vtype <= SB_VT_I64, "LIT_I64 node %d: vtype %d is not BOOL, I32 or I64", i, nd.vtype);
+        break;
+      case SB_OP_LIT_F64: SB_REQUIRE(nd.vtype == SB_VT_F64, "LIT_F64 node %d: vtype %d is not F64", i, nd.vtype); break;
+      case SB_OP_LIT_NULL:
+        SB_REQUIRE(nd.vtype >= SB_VT_BOOL && nd.vtype <= SB_VT_F64, "LIT_NULL node %d: unknown vtype %d", i, nd.vtype);
+        break;
       case SB_OP_ADD: case SB_OP_SUB: case SB_OP_MUL: case SB_OP_DIV:
       case SB_OP_EQ: case SB_OP_NE: case SB_OP_LT: case SB_OP_LE: case SB_OP_GT: case SB_OP_GE:
-      case SB_OP_AND: case SB_OP_OR:
+      case SB_OP_AND: case SB_OP_OR: {
         SB_REQUIRE(depth >= 2, "expression stack underflow at node %d", i);
+        int32_t want;
+        if (nd.op == SB_OP_DIV) {
+          want = SB_VT_F64;
+          SB_REQUIRE(nd.vtype == SB_VT_F64, "DIV node %d: vtype %d is not F64", i, nd.vtype);
+        } else if (nd.op >= SB_OP_ADD && nd.op <= SB_OP_MUL) {
+          want = nd.vtype;
+          SB_REQUIRE(nd.vtype >= SB_VT_I32 && nd.vtype <= SB_VT_F64, "arithmetic node %d: vtype %d is not numeric", i, nd.vtype);
+        } else if (nd.op >= SB_OP_EQ && nd.op <= SB_OP_GE) {
+          want = nd.arg;
+          SB_REQUIRE(nd.vtype == SB_VT_BOOL, "comparison node %d: vtype %d is not BOOL", i, nd.vtype);
+        } else {
+          want = SB_VT_BOOL;
+          SB_REQUIRE(nd.vtype == SB_VT_BOOL, "AND / OR node %d: vtype %d is not BOOL", i, nd.vtype);
+        }
+        SB_REQUIRE(operand_ok(depth - 2, want) && operand_ok(depth - 1, want), "node %d (op %d): operands of vtype %d and %d, expected %d", i,
+                   nd.op, vt[depth - 2], vt[depth - 1], want);
+        depth -= 2;
+        break;
+      }
+      case SB_OP_NEG: case SB_OP_NOT: case SB_OP_ISNULL: case SB_OP_ISNOTNULL:
+      case SB_OP_CAST_F64: case SB_OP_CAST_I64: case SB_OP_CAST_I32: {
+        SB_REQUIRE(depth >= 1, "expression stack underflow at node %d", i);
+        const int32_t src = vt[depth - 1];
+        if (nd.op == SB_OP_NEG) {
+          SB_REQUIRE(nd.vtype >= SB_VT_I32 && nd.vtype <= SB_VT_F64 && operand_ok(depth - 1, nd.vtype), "NEG node %d: vtype %d over an operand of vtype %d", i,
+                     nd.vtype, src);
+        } else if (nd.op == SB_OP_NOT) {
+          SB_REQUIRE(nd.vtype == SB_VT_BOOL && operand_ok(depth - 1, SB_VT_BOOL), "NOT node %d: vtype %d over an operand of vtype %d", i, nd.vtype, src);
+        } else if (nd.op == SB_OP_ISNULL || nd.op == SB_OP_ISNOTNULL) {
+          SB_REQUIRE(nd.vtype == SB_VT_BOOL, "IS [NOT] NULL node %d: vtype %d is not BOOL", i, nd.vtype);
+        } else {
+          res = nd.op == SB_OP_CAST_F64 ? SB_VT_F64 : nd.op == SB_OP_CAST_I64 ? SB_VT_I64 : SB_VT_I32;
+          SB_REQUIRE(nd.vtype == res, "CAST node %d: vtype %d, expected %d", i, nd.vtype, res);
+          SB_REQUIRE(nd.arg >= SB_VT_BOOL && nd.arg <= SB_VT_F64 && operand_ok(depth - 1, nd.arg),
+                     "CAST node %d: arg (source class) %d but the operand has vtype %d", i, nd.arg, src);
+        }
         depth--;
         break;
-      case SB_OP_NEG: case SB_OP_NOT: case SB_OP_ISNULL: case SB_OP_ISNOTNULL:
-      case SB_OP_CAST_F64: case SB_OP_CAST_I64: case SB_OP_CAST_I32:
-        SB_REQUIRE(depth >= 1, "expression stack underflow at node %d", i);
-        break;
+      }
       default: fail(SB_ERR_INVALID, "unknown expression op %d at node %d", nd.op, i);
     }
-    SB_REQUIRE(depth <= EXPR_STACK, "expression needs more than %d stack slots", EXPR_STACK);
+    SB_REQUIRE(depth < EXPR_STACK, "expression needs more than %d stack slots", EXPR_STACK);
+    vt[depth] = res;
+    null_lit[depth] = nd.op == SB_OP_LIT_NULL;
+    depth++;
   }
   SB_REQUIRE(depth == 1, "expression leaves %d values on the stack", depth);
 }
@@ -105,8 +160,8 @@ bool expr_nullable(const sb_table *in, const sb_expr &e) {
   return false;
 }
 
+// `e` has passed expr_validate
 static DevProg build_prog(const sb_table *in, const sb_expr &e) {
-  expr_validate(in, e);
   DevProg p;
   p.n = e.n;
   p.ncols = 0;
@@ -355,6 +410,7 @@ __global__ void __launch_bounds__(256) simple_predicate_kernel(const __grid_cons
 }
 
 void eval_predicate(const sb_table *in, const sb_expr &pred, uint8_t *mask, cudaStream_t st) {
+  expr_validate(in, pred);   // before the fast path: its matcher trusts the program (a DECIMAL term would compare unscaled values)
   int64_t n = in->nrows;
   if (n == 0) return;
   KernelTimer kt("filter_project", st);
@@ -378,6 +434,7 @@ Column eval_projection(const sb_table *in, const sb_expr &e, const int64_t *sel,
     if (!sel) return column_share(in->cols[col]);
     return gather_column(in->cols[col], sel, nout, false, st);
   }
+  expr_validate(in, e);
   DevProg p = build_prog(in, e);
   SB_REQUIRE(e.out_type != SB_STRING && type_width(e.out_type) > 0, "bad projection result type %d", e.out_type);
   Column r = column_alloc(e.out_type, 0, nout, expr_nullable(in, e), st);

@@ -14,9 +14,9 @@ bool expr_is_column(const sb_expr &e, int *col);
 // can the result contain NULLs?
 bool expr_nullable(const sb_table *in, const sb_expr &e);
 
-// mask[i] = 1 when the predicate is TRUE (not NULL) for row i
+// mask[i] = 1 when the predicate is TRUE (not NULL) for row i; validates the program first (also for an empty table)
 void eval_predicate(const sb_table *in, const sb_expr &pred, uint8_t *mask_dev, cudaStream_t st);
-// materialises the expression for rows sel[0..nout) (sel == nullptr -> rows 0..nout)
+// materialises the expression for rows sel[0..nout) (sel == nullptr -> rows 0..nout); validates it unless it is a bare column
 Column eval_projection(const sb_table *in, const sb_expr &e, const int64_t *sel, int64_t nout, cudaStream_t st);
 
 }  // namespace sb

@@ -822,10 +822,7 @@ int sb_join_build_filtered(const sb_table *build, const int32_t *key_cols, int32
   }
   JoinKeys k = make_join_keys(ev.view ? ev.view : build, key_cols, nkeys, nullptr);
   Scratch mask(filter ? n + 16 : 0, st);
-  if (filter) {
-    expr_validate(build, *filter);
-    if (n > 0) eval_predicate(build, *filter, mask.as<uint8_t>(), st);
-  }
+  if (filter) eval_predicate(build, *filter, mask.as<uint8_t>(), st);   // validates the program even when n == 0
   sb_hash_table *ht = new sb_hash_table();
   ht->st = st;
   ht->nkeys = nkeys;
@@ -1366,9 +1363,8 @@ int sb_join_probe_condition(const sb_hash_table *ht, const sb_table *probe, cons
   // is built again below from indices; here only the mask is taken from it
   struct Guard { sb_table *&t; ~Guard() { if (t) sb::table_free(t); } } g1{pairs_tbl};
   const int64_t npairs = pairs_tbl->nrows;
-  expr_validate(pairs_tbl, *condition);
   Scratch mask(npairs + 16, st);
-  if (npairs > 0) eval_predicate(pairs_tbl, *condition, mask.as<uint8_t>(), st);
+  eval_predicate(pairs_tbl, *condition, mask.as<uint8_t>(), st);   // validates the program even when there is no pair
   // pair indices: the same kernels again with index outputs only (count + fill), cheaper than carrying row ids through the gather
   EncodedView key_view;
   JoinKeys k = make_join_keys(probe_key_source(ht, probe, key_cols, nkeys, st, key_view), key_cols, nkeys, ht);
