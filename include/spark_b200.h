@@ -112,7 +112,7 @@ int sb_profile_dump(char *buf, int32_t len);   /* "name=total_ms/launches;..." o
  *                       input (the GPU analogue of WholeStageCodegenExec + Janino), 0 = always run the generic kernels
  *   "agg_rtc_min_rows"  inputs with fewer rows run the generic kernels (default 2^20)
  *   "agg_tier"          0 auto, 1 dictionary tier only, 2 shared-memory tier only
- *   "agg_staged", "agg_verbose", "expr_interpret_only", "regroup_ldst", "exchange_nccl"   0/1
+ *   "agg_verbose", "expr_interpret_only", "regroup_ldst", "exchange_nccl"   0/1
  *   "join_cand"         join candidate pass: 0 = 16 consecutive rows per thread, 1..3 = lane-strided geometries (default 2)
  *   "sort_variant"      onesweep tile geometry 0..5 (default 4 = 384 threads x 12 keys) */
 int sb_config_set(const char *key, int64_t value);

@@ -26,8 +26,6 @@ constexpr int AGG_MAX_WORDS = 4;
 constexpr int AGG_MAX_TERMS = 4;
 constexpr int AGG_MAX_FACT = 3;
 constexpr int AGG_MAX_COLS = 20;      // distinct input columns of one plan
-constexpr int AGG_MAX_STAGED = 32;    // distinct buffers (values + validity bitmaps) a staged tile may hold
-constexpr int AGG_MAX_STAGES = 4;
 constexpr int AGG_PROBE_LIMIT = 64;
 constexpr uint64_t EMPTY_KEY = 0xFFFFFFFFFFFFFFFFull;
 
@@ -56,13 +54,6 @@ struct PlanMeta {
 struct ColRef {              // where one input buffer lives
   const void *data;          // HBM
   const uint8_t *valid;      // HBM validity bitmap or nullptr
-  int32_t soff;              // staged path: byte offset of the tile inside a shared-memory stage
-  int32_t svoff;             // ... of the validity tile, or -1
-};
-struct StagedBuf {           // one buffer the TMA producer copies per tile
-  const uint8_t *base;
-  int32_t bytes_per_tile;    // multiple of 16
-  int32_t soff;              // 128-byte aligned
 };
 struct KeyExtra {            // wide-key placement (multi-word keys only)
   int32_t word, null_word, hi_word, hi_shift;
@@ -74,8 +65,7 @@ struct AggArgs {
   int64_t term_lit[AGG_MAX_TERMS];               // int64 value or double bits
   KeyExtra key_extra[AGG_MAX_KEYS];
   double fac_lit[AGG_MAX_SLOTS][AGG_MAX_FACT];
-  int32_t nwords, nstaged, stage_bytes, nstages;
-  StagedBuf staged[AGG_MAX_STAGED];
+  int32_t nwords;
   uint64_t *tkeys;       // [nwords][cap + 2]   slot cap = NULL key, slot cap+1 = key equal to the EMPTY sentinel
   uint64_t *tacc;        // [nslots][cap + 2]
   int32_t *flags;        // [0] abort (table too small), [1] NULL-key slot used, [2] sentinel-key slot used,
@@ -166,73 +156,57 @@ __device__ __forceinline__ int64_t table_slot(const AggArgs &a, uint64_t key, in
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Tile processing.  A thread owns ITEMS rows of a tile (row k = row0 + k*AGG_THREADS, coalesced per k).
-//   * direct path: row0 is the absolute row, pointers are the column buffers in HBM; FULL tiles use unclamped loads
-//     (LDG [base + k*stride] with immediate offsets, all ITEMS loads of a column in flight together);
-//   * staged path: the block's TMA producer copied the tile of every referenced buffer into shared memory, row0 is the
-//     thread's row inside the tile and pointers are `stage + soff`.
+// Tile processing.  A thread owns ITEMS rows of a tile (row k = row0 + k*AGG_THREADS, coalesced per k); row0 is the absolute
+// row and pointers are the column buffers in HBM.  FULL tiles use unclamped loads (LDG [base + k*stride] with immediate
+// offsets, all ITEMS loads of a column in flight together).
 // Every warp-uniform decision (column type, factor mode, accumulator kind) is taken OUTSIDE the unrolled row loop, and
 // with a StaticPlan it is taken by the compiler.
 // ---------------------------------------------------------------------------------------------------------
 struct TileCtx {
-  const uint8_t *stage;   // shared-memory stage (staged path) or nullptr
   int64_t row0;
-  int64_t last;           // clamp for partial tiles (direct path only)
+  int64_t last;           // clamp for partial tiles
 };
-template <bool STAGED>
-__device__ __forceinline__ const void *tile_ptr(const TileCtx &t, const ColRef &c) {
-  return STAGED ? (const void *)(t.stage + c.soff) : c.data;
-}
-template <bool STAGED>
-__device__ __forceinline__ const uint8_t *tile_valid(const TileCtx &t, const ColRef &c) {
-  return STAGED ? t.stage + c.svoff : c.valid;
-}
 
-// NC = the buffer is read-only HBM: loads go through ld.global.nc (__ldg), which tells the compiler they cannot alias the
+// Column buffers are read-only HBM: loads go through ld.global.nc (__ldg), which tells the compiler they cannot alias the
 // shared-memory accumulator stores, so it is free to hoist the loads of later slots above earlier accumulations and to
 // merge repeated loads of the same column (a static plan's straight-line code then keeps a whole tile's loads in flight).
-template <bool NC, typename T>
-__device__ __forceinline__ T tile_load(const T *p) {
-  if (NC) return __ldg(p);
-  return *p;
-}
-template <int ITEMS, bool FULL, bool NC, typename T>
+template <int ITEMS, bool FULL, typename T>
 __device__ __forceinline__ void load_batch_as_i64(const void *__restrict__ data, const TileCtx &t, int64_t (&out)[ITEMS]) {
   const T *p = (const T *)data + t.row0;
 #pragma unroll
   for (int k = 0; k < ITEMS; k++) {
-    if (FULL) out[k] = (int64_t)tile_load<NC>(p + k * AGG_THREADS);
+    if (FULL) out[k] = (int64_t)__ldg(p + k * AGG_THREADS);
     else {
       int64_t r = t.row0 + (int64_t)k * AGG_THREADS;
-      out[k] = (int64_t)tile_load<NC>((const T *)data + (r < t.last ? r : t.last));
+      out[k] = (int64_t)__ldg((const T *)data + (r < t.last ? r : t.last));
     }
   }
 }
-template <int ITEMS, bool FULL, bool NC>
+template <int ITEMS, bool FULL>
 __device__ __forceinline__ void load_i64_batch(const void *__restrict__ data, int32_t type, const TileCtx &t, int64_t (&out)[ITEMS]) {
   switch (type) {
-    case SB_BOOL: load_batch_as_i64<ITEMS, FULL, NC, uint8_t>(data, t, out); break;
-    case SB_INT8: load_batch_as_i64<ITEMS, FULL, NC, int8_t>(data, t, out); break;
-    case SB_INT16: load_batch_as_i64<ITEMS, FULL, NC, int16_t>(data, t, out); break;
-    case SB_INT32: case SB_DATE32: case SB_FLOAT32: load_batch_as_i64<ITEMS, FULL, NC, int32_t>(data, t, out); break;
-    default: load_batch_as_i64<ITEMS, FULL, NC, int64_t>(data, t, out); break;
+    case SB_BOOL: load_batch_as_i64<ITEMS, FULL, uint8_t>(data, t, out); break;
+    case SB_INT8: load_batch_as_i64<ITEMS, FULL, int8_t>(data, t, out); break;
+    case SB_INT16: load_batch_as_i64<ITEMS, FULL, int16_t>(data, t, out); break;
+    case SB_INT32: case SB_DATE32: case SB_FLOAT32: load_batch_as_i64<ITEMS, FULL, int32_t>(data, t, out); break;
+    default: load_batch_as_i64<ITEMS, FULL, int64_t>(data, t, out); break;
   }
 }
-template <int ITEMS, bool FULL, bool NC>
+template <int ITEMS, bool FULL>
 __device__ __forceinline__ void load_f64_batch(const void *__restrict__ data, int32_t type, const TileCtx &t, double (&out)[ITEMS]) {
   if (type == SB_FLOAT64) {
     const double *p = (const double *)data + t.row0;
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) {
-      if (FULL) out[k] = tile_load<NC>(p + k * AGG_THREADS);
+      if (FULL) out[k] = __ldg(p + k * AGG_THREADS);
       else {
         int64_t r = t.row0 + (int64_t)k * AGG_THREADS;
-        out[k] = tile_load<NC>((const double *)data + (r < t.last ? r : t.last));
+        out[k] = __ldg((const double *)data + (r < t.last ? r : t.last));
       }
     }
   } else {
     int64_t x[ITEMS];
-    load_i64_batch<ITEMS, FULL, NC>(data, type, t, x);
+    load_i64_batch<ITEMS, FULL>(data, type, t, x);
     if (type == SB_FLOAT32) {
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) out[k] = (double)__int_as_float((int32_t)x[k]);
@@ -242,14 +216,14 @@ __device__ __forceinline__ void load_f64_batch(const void *__restrict__ data, in
     }
   }
 }
-template <int ITEMS, bool FULL, bool NC>
+template <int ITEMS, bool FULL>
 __device__ __forceinline__ void load_valid_batch(const uint8_t *__restrict__ valid, const TileCtx &t, bool (&out)[ITEMS]) {
   uint8_t b[ITEMS];
 #pragma unroll
   for (int k = 0; k < ITEMS; k++) {
     int64_t r = t.row0 + (int64_t)k * AGG_THREADS;
     if (!FULL) r = r < t.last ? r : t.last;
-    b[k] = tile_load<NC>(valid + (r >> 3));
+    b[k] = __ldg(valid + (r >> 3));
   }
 #pragma unroll
   for (int k = 0; k < ITEMS; k++) {
@@ -260,13 +234,13 @@ __device__ __forceinline__ void load_valid_batch(const uint8_t *__restrict__ val
 }
 
 // fused FilterExec: conjunction of column-vs-literal terms (a NULL comparison drops the row)
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void apply_filter_terms(const AggArgs &a, const TileCtx &t, bool (&keep)[ITEMS]) {
   const PlanMeta &m = P::meta(a);
   plan_for<P>(m.nterms, [&](int i) {
     if (m.term_valid[i]) {
       bool valid[ITEMS];
-      load_valid_batch<ITEMS, FULL, !STAGED>(tile_valid<STAGED>(t, a.col[m.term_col[i]]), t, valid);
+      load_valid_batch<ITEMS, FULL>(a.col[m.term_col[i]].valid, t, valid);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) keep[k] = keep[k] && valid[k];
     }
@@ -275,7 +249,7 @@ __device__ __forceinline__ void apply_filter_terms(const AggArgs &a, const TileC
     int c[ITEMS];
     if (m.term_f64[i]) {
       double x[ITEMS];
-      load_f64_batch<ITEMS, FULL, !STAGED>(tile_ptr<STAGED>(t, a.col[m.term_col[i]]), m.term_type[i], t, x);
+      load_f64_batch<ITEMS, FULL>(a.col[m.term_col[i]].data, m.term_type[i], t, x);
       const double y = __longlong_as_double(a.term_lit[i]);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) {   // SQLOrderingUtil.compareDoubles
@@ -284,7 +258,7 @@ __device__ __forceinline__ void apply_filter_terms(const AggArgs &a, const TileC
       }
     } else {
       int64_t x[ITEMS];
-      load_i64_batch<ITEMS, FULL, !STAGED>(tile_ptr<STAGED>(t, a.col[m.term_col[i]]), m.term_type[i], t, x);
+      load_i64_batch<ITEMS, FULL>(a.col[m.term_col[i]].data, m.term_type[i], t, x);
       const int64_t lit = a.term_lit[i];
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) c[k] = x[k] == lit ? 0 : (x[k] < lit ? -1 : 1);
@@ -303,10 +277,10 @@ __device__ __forceinline__ void apply_filter_terms(const AggArgs &a, const TileC
 }
 
 // value of factor f of slot s for the thread's rows: col | lit-col | lit+col | col-lit
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void factor_batch(const AggArgs &a, int s, int f, const TileCtx &t, double (&y)[ITEMS]) {
   const PlanMeta &m = P::meta(a);
-  load_f64_batch<ITEMS, FULL, !STAGED>(tile_ptr<STAGED>(t, a.col[m.f_col[s][f]]), m.f_type[s][f], t, y);
+  load_f64_batch<ITEMS, FULL>(a.col[m.f_col[s][f]].data, m.f_type[s][f], t, y);
   const int mode = m.f_mode[s][f];
   if (mode == F_COL) return;
   const double lit = a.fac_lit[s][f];
@@ -326,20 +300,20 @@ __device__ __forceinline__ void factor_batch(const AggArgs &a, int s, int f, con
   }
 }
 // left-deep product of the slot's factors, evaluated in the reference's order ((f0*f1)*f2), no FMA contraction
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void product_batch(const AggArgs &a, int s, const TileCtx &t, double (&y)[ITEMS]) {
   const PlanMeta &m = P::meta(a);
-  factor_batch<P, ITEMS, FULL, STAGED>(a, s, 0, t, y);
+  factor_batch<P, ITEMS, FULL>(a, s, 0, t, y);
   plan_for<P>(m.slot_nf[s] - 1, [&](int f1) {
     double z[ITEMS];
-    factor_batch<P, ITEMS, FULL, STAGED>(a, s, f1 + 1, t, z);
+    factor_batch<P, ITEMS, FULL>(a, s, f1 + 1, t, z);
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) y[k] = __dmul_rn(y[k], z[k]);
   });
 }
 
 // 64-bit accumulator payload of slot s for the thread's rows
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void slot_values(const AggArgs &a, int s, const TileCtx &t, uint64_t (&v)[ITEMS]) {
   const PlanMeta &m = P::meta(a);
   const int kind = m.slot_kind[s], xform = m.slot_xform[s];
@@ -348,7 +322,7 @@ __device__ __forceinline__ void slot_values(const AggArgs &a, int s, const TileC
     for (int k = 0; k < ITEMS; k++) v[k] = 1;
   } else if (kind == K_ADD_F64 || xform == X_DOUBLE) {
     double y[ITEMS];
-    product_batch<P, ITEMS, FULL, STAGED>(a, s, t, y);
+    product_batch<P, ITEMS, FULL>(a, s, t, y);
     if (xform == X_DOUBLE) {   // order-preserving bits for min/max, NaN canonical (largest)
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) {
@@ -361,7 +335,7 @@ __device__ __forceinline__ void slot_values(const AggArgs &a, int s, const TileC
     }
   } else {
     int64_t x[ITEMS];
-    load_i64_batch<ITEMS, FULL, !STAGED>(tile_ptr<STAGED>(t, a.col[m.f_col[s][0]]), m.f_type[s][0], t, x);
+    load_i64_batch<ITEMS, FULL>(a.col[m.f_col[s][0]].data, m.f_type[s][0], t, x);
     const uint64_t flip = xform == X_SIGNED ? 0x8000000000000000ull : 0ull;
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) v[k] = (uint64_t)x[k] ^ flip;
@@ -369,14 +343,14 @@ __device__ __forceinline__ void slot_values(const AggArgs &a, int s, const TileC
 }
 
 // rows whose inputs are NULL do not contribute (Sum.scala:113, Count.scala:94): ok[k] &= all factor columns valid
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void slot_input_valid(const AggArgs &a, int s, const TileCtx &t, bool (&ok)[ITEMS]) {
   const PlanMeta &m = P::meta(a);
   if (!m.slot_anyvalid[s]) return;
   plan_for<P>(m.slot_nf[s], [&](int f) {
     if (m.f_valid[s][f]) {
       bool valid[ITEMS];
-      load_valid_batch<ITEMS, FULL, !STAGED>(tile_valid<STAGED>(t, a.col[m.f_col[s][f]]), t, valid);
+      load_valid_batch<ITEMS, FULL>(a.col[m.f_col[s][f]].valid, t, valid);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) ok[k] = ok[k] && valid[k];
     }
@@ -385,7 +359,7 @@ __device__ __forceinline__ void slot_input_valid(const AggArgs &a, int s, const 
 
 // General accumulate: dst[k] >= 0: HBM table slot; doff[k] >= 0: offset of the row's group in the lane-private
 // shared-memory accumulators (dictionary hit); both negative: row filtered out.
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void accumulate_slots(const AggArgs &a, const TileCtx &t, const int64_t (&dst)[ITEMS], const int (&doff)[ITEMS],
                                                  uint64_t *acc, int64_t stride) {
   const PlanMeta &m = P::meta(a);
@@ -394,8 +368,8 @@ __device__ __forceinline__ void accumulate_slots(const AggArgs &a, const TileCtx
     bool ok[ITEMS];
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) ok[k] = dst[k] >= 0 || doff[k] >= 0;
-    slot_input_valid<P, ITEMS, FULL, STAGED>(a, s, t, ok);
-    slot_values<P, ITEMS, FULL, STAGED>(a, s, t, v);
+    slot_input_valid<P, ITEMS, FULL>(a, s, t, ok);
+    slot_values<P, ITEMS, FULL>(a, s, t, v);
     uint64_t *sacc = acc + (size_t)s * AGG_THREADS;
     uint64_t *gacc = a.tacc + (int64_t)s * stride;
     switch (m.slot_kind[s]) {
@@ -431,7 +405,7 @@ __device__ __forceinline__ void accumulate_slots(const AggArgs &a, const TileCtx
 // phase 2 walks rows outer / slots inner: for one row the slots' accumulators are acc + s*AGG_THREADS + doff[k] with s a
 // compile-time constant, i.e. provably distinct addresses, so their LDS/op/STS chains overlap instead of forming one
 // long read-after-write chain through shared memory.
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void accumulate_slots_dict(const AggArgs &a, const TileCtx &t, const int (&doff)[ITEMS], uint64_t *acc, int trash) {
   const PlanMeta &m = P::meta(a);
   if constexpr (P::kStatic) {
@@ -442,7 +416,7 @@ __device__ __forceinline__ void accumulate_slots_dict(const AggArgs &a, const Ti
       const int cls = m.slot_cls[s];
       if (cls == CLS_F64_PRODUCT) {
         double y[ITEMS];
-        product_batch<P, ITEMS, FULL, STAGED>(a, s, t, y);
+        product_batch<P, ITEMS, FULL>(a, s, t, y);
 #pragma unroll
         for (int k = 0; k < ITEMS; k++) v[s][k] = (uint64_t)__double_as_longlong(y[k]);
       } else if (cls == CLS_ONE) {
@@ -452,8 +426,8 @@ __device__ __forceinline__ void accumulate_slots_dict(const AggArgs &a, const Ti
         bool ok[ITEMS];
 #pragma unroll
         for (int k = 0; k < ITEMS; k++) ok[k] = true;
-        slot_input_valid<P, ITEMS, FULL, STAGED>(a, s, t, ok);
-        slot_values<P, ITEMS, FULL, STAGED>(a, s, t, v[s]);
+        slot_input_valid<P, ITEMS, FULL>(a, s, t, ok);
+        slot_values<P, ITEMS, FULL>(a, s, t, v[s]);
 #pragma unroll
         for (int k = 0; k < ITEMS; k++) nullbits[s] |= ok[k] ? 0u : (1u << k);
       }
@@ -477,7 +451,7 @@ __device__ __forceinline__ void accumulate_slots_dict(const AggArgs &a, const Ti
     const int cls = m.slot_cls[s];
     if (cls == CLS_F64_PRODUCT) {
       double y[ITEMS];
-      product_batch<P, ITEMS, FULL, STAGED>(a, s, t, y);
+      product_batch<P, ITEMS, FULL>(a, s, t, y);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) {
         double *p = (double *)(sacc + doff[k]);
@@ -491,8 +465,8 @@ __device__ __forceinline__ void accumulate_slots_dict(const AggArgs &a, const Ti
       bool ok[ITEMS];
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) ok[k] = true;
-      slot_input_valid<P, ITEMS, FULL, STAGED>(a, s, t, ok);
-      slot_values<P, ITEMS, FULL, STAGED>(a, s, t, v);
+      slot_input_valid<P, ITEMS, FULL>(a, s, t, ok);
+      slot_values<P, ITEMS, FULL>(a, s, t, v);
       switch (m.slot_kind[s]) {
 #define SB_ACCD(EXPR) _Pragma("unroll") for (int k = 0; k < ITEMS; k++) { uint64_t *p = sacc + (ok[k] ? doff[k] : trash); EXPR; }
         case K_ADD_F64: SB_ACCD(*(double *)p = __dadd_rn(*(double *)p, __longlong_as_double((int64_t)v[k]))) break;
@@ -506,9 +480,9 @@ __device__ __forceinline__ void accumulate_slots_dict(const AggArgs &a, const Ti
 }
 
 // Shared memory of the update kernels: uint64 dict_keys[D]; uint64 fill; uint64 acc[(D + 1) * nslots][AGG_THREADS]
-// (last group = trash); the staged kernel puts the column stages and the mbarriers in front.
+// (last group = trash).
 // keep / packed group key / special-slot class of the thread's rows
-template <class P, int ITEMS, bool FULL, bool STAGED>
+template <class P, int ITEMS, bool FULL>
 __device__ __forceinline__ void tile_keys(const AggArgs &a, const TileCtx &t, bool (&keep)[ITEMS], uint64_t (&key)[ITEMS], int (&special)[ITEMS]) {
   const PlanMeta &m = P::meta(a);
 #pragma unroll
@@ -518,17 +492,17 @@ __device__ __forceinline__ void tile_keys(const AggArgs &a, const TileCtx &t, bo
   }
   if (m.has_mask) {
     int64_t x[ITEMS];
-    load_batch_as_i64<ITEMS, FULL, !STAGED, uint8_t>(tile_ptr<STAGED>(t, a.col[m.mask_col]), t, x);
+    load_batch_as_i64<ITEMS, FULL, uint8_t>(a.col[m.mask_col].data, t, x);
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) keep[k] = keep[k] && x[k] != 0;
   }
-  apply_filter_terms<P, ITEMS, FULL, STAGED>(a, t, keep);
+  apply_filter_terms<P, ITEMS, FULL>(a, t, keep);
   // ---- group key packing --------------------------------------------------------------------------------
 #pragma unroll
   for (int k = 0; k < ITEMS; k++) special[k] = 0;
   if (m.single64) {
     int64_t x[ITEMS];
-    load_batch_as_i64<ITEMS, FULL, !STAGED, int64_t>(tile_ptr<STAGED>(t, a.col[m.key_col[0]]), t, x);      // raw 64-bit words
+    load_batch_as_i64<ITEMS, FULL, int64_t>(a.col[m.key_col[0]].data, t, x);      // raw 64-bit words
     if (m.key_type[0] == SB_FLOAT64) {   // NormalizeFloatingNumbers: -0.0 -> 0.0, NaN canonical
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) {
@@ -543,7 +517,7 @@ __device__ __forceinline__ void tile_keys(const AggArgs &a, const TileCtx &t, bo
     }
     if (m.key_valid[0]) {
       bool valid[ITEMS];
-      load_valid_batch<ITEMS, FULL, !STAGED>(tile_valid<STAGED>(t, a.col[m.key_col[0]]), t, valid);
+      load_valid_batch<ITEMS, FULL>(a.col[m.key_col[0]].valid, t, valid);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) special[k] = valid[k] ? special[k] : 1;
     }
@@ -551,7 +525,7 @@ __device__ __forceinline__ void tile_keys(const AggArgs &a, const TileCtx &t, bo
     plan_for<P>(m.nkeys, [&](int i) {
       const int kt = m.key_type[i], bits = m.key_bits[i], shift = m.key_shift[i];
       int64_t x[ITEMS];
-      load_i64_batch<ITEMS, FULL, !STAGED>(tile_ptr<STAGED>(t, a.col[m.key_col[i]]), kt, t, x);
+      load_i64_batch<ITEMS, FULL>(a.col[m.key_col[i]].data, kt, t, x);
       if (kt == SB_FLOAT32) {
 #pragma unroll
         for (int k = 0; k < ITEMS; k++) {
@@ -563,7 +537,7 @@ __device__ __forceinline__ void tile_keys(const AggArgs &a, const TileCtx &t, bo
       if (m.key_valid[i]) {
         const int nshift = m.key_nshift[i];
         bool valid[ITEMS];
-        load_valid_batch<ITEMS, FULL, !STAGED>(tile_valid<STAGED>(t, a.col[m.key_col[i]]), t, valid);
+        load_valid_batch<ITEMS, FULL>(a.col[m.key_col[i]].valid, t, valid);
 #pragma unroll
         for (int k = 0; k < ITEMS; k++) key[k] |= valid[k] ? ((uint64_t)x[k] & vmask) << shift : 1ull << nshift;
       } else {
@@ -574,14 +548,14 @@ __device__ __forceinline__ void tile_keys(const AggArgs &a, const TileCtx &t, bo
   }
 }
 
-template <class P, int ITEMS, bool FULL, bool STAGED, bool YIELD = false, int D = AGG_DICT>
+template <class P, int ITEMS, bool FULL, bool YIELD = false, int D = AGG_DICT>
 __device__ __forceinline__ bool process_tile(const AggArgs &a, const TileCtx &t, uint64_t *dict_keys, uint64_t *acc, int tid, int64_t stride) {
   const PlanMeta &m = P::meta(a);
   const int ns = m.nslots;
   bool keep[ITEMS];
   uint64_t key[ITEMS];
   int special[ITEMS];
-  tile_keys<P, ITEMS, FULL, STAGED>(a, t, keep, key, special);
+  tile_keys<P, ITEMS, FULL>(a, t, keep, key, special);
   // ---- where does each row accumulate? ---------------------------------------------------------------------
   int64_t dst[ITEMS];
   int doff[ITEMS];
@@ -646,15 +620,15 @@ __device__ __forceinline__ bool process_tile(const AggArgs &a, const TileCtx &t,
     if (!__all_sync(0xffffffffu, all_dict)) return false;
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) doff[k] = doff[k] >= 0 ? doff[k] : trash;
-    accumulate_slots_dict<P, ITEMS, FULL, STAGED>(a, t, doff, acc, trash);
+    accumulate_slots_dict<P, ITEMS, FULL>(a, t, doff, acc, trash);
     return true;
   }
   if (__all_sync(0xffffffffu, all_dict)) {
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) doff[k] = doff[k] >= 0 ? doff[k] : trash;
-    accumulate_slots_dict<P, ITEMS, FULL, STAGED>(a, t, doff, acc, trash);
+    accumulate_slots_dict<P, ITEMS, FULL>(a, t, doff, acc, trash);
   } else {
-    accumulate_slots<P, ITEMS, FULL, STAGED>(a, t, dst, doff, acc, stride);
+    accumulate_slots<P, ITEMS, FULL>(a, t, dst, doff, acc, stride);
   }
   return true;
 }
@@ -727,7 +701,7 @@ __device__ __forceinline__ void prefetch_tile(const AggArgs &a, int64_t row0) {
 // 28 warps per SM with D = 4 against 16 with D = 8 -- the 4-group query runs faster at the higher occupancy -- and a 5..8-group
 // input costs one extra launch.
 enum { AGG_MODE_PLAIN = 0, AGG_MODE_YIELD = 1, AGG_MODE_TAKEOVER = 2 };
-template <class P, int ITEMS, bool PREFETCH = false, int MODE = AGG_MODE_PLAIN, bool FAT = false, int D = AGG_DICT>
+template <class P, int ITEMS, bool PREFETCH = false, int MODE = AGG_MODE_PLAIN, int D = AGG_DICT>
 __global__ void __launch_bounds__(AGG_THREADS) agg_update_kernel(const __grid_constant__ AggArgs a) {
   extern __shared__ __align__(128) uint64_t sm_direct[];
   uint64_t *dict_keys = sm_direct;
@@ -747,19 +721,17 @@ __global__ void __launch_bounds__(AGG_THREADS) agg_update_kernel(const __grid_co
   auto one_tile = [&](int64_t base, int64_t next) -> bool {   // false: this warp yields (the tile is untouched)
     stop = *(volatile int32_t *)a.flags;                       // another block found the table too small: give up early
     if (YIELD) stop |= *yield_flag;                            // somebody met rows this tier should not handle
-    TileCtx t{nullptr, base + tid, a.n - 1};
+    TileCtx t{base + tid, a.n - 1};
     if (PREFETCH && next + TILE <= a.n) prefetch_tile<P, ITEMS>(a, next + tid);
-    if (FAT && a.gate == 3) {   // never taken; see SB_AGG_Q1_VARIANT in aggregate.cu
-      process_tile<P, ITEMS, true, false, false, D>(a, t, dict_keys, acc, tid, stride);
-    } else if constexpr (YIELD) {
-      const bool done = base + TILE <= a.n ? process_tile<P, ITEMS, true, false, true, D>(a, t, dict_keys, acc, tid, stride)
-                                           : process_tile<P, ITEMS, false, false, true, D>(a, t, dict_keys, acc, tid, stride);
+    if constexpr (YIELD) {
+      const bool done = base + TILE <= a.n ? process_tile<P, ITEMS, true, true, D>(a, t, dict_keys, acc, tid, stride)
+                                           : process_tile<P, ITEMS, false, true, D>(a, t, dict_keys, acc, tid, stride);
       if (!done) {
         *yield_flag = 1;
         return false;
       }
-    } else if (base + TILE <= a.n) process_tile<P, ITEMS, true, false, false, D>(a, t, dict_keys, acc, tid, stride);
-    else process_tile<P, ITEMS, false, false, false, D>(a, t, dict_keys, acc, tid, stride);
+    } else if (base + TILE <= a.n) process_tile<P, ITEMS, true, false, D>(a, t, dict_keys, acc, tid, stride);
+    else process_tile<P, ITEMS, false, false, D>(a, t, dict_keys, acc, tid, stride);
     return true;
   };
   if constexpr (MODE == AGG_MODE_TAKEOVER) {
@@ -834,7 +806,7 @@ __device__ __forceinline__ void process_tile_smem(const AggArgs &a, const TileCt
   bool keep[ITEMS];
   uint64_t key[ITEMS];
   int special[ITEMS];
-  tile_keys<P, ITEMS, FULL, false>(a, t, keep, key, special);
+  tile_keys<P, ITEMS, FULL>(a, t, keep, key, special);
   const uint32_t C = (uint32_t)a.scap, cmask = C - 1, fill_limit = C - (C >> 2);
   volatile uint32_t *vctl = sctl;
   // control words change under our feet: take one reading per warp so that warp-collective code below stays converged
@@ -926,8 +898,8 @@ __device__ __forceinline__ void process_tile_smem(const AggArgs &a, const TileCt
     bool ok[ITEMS];
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) ok[k] = dst[k] >= 0 || soff[k] >= 0;
-    slot_input_valid<P, ITEMS, FULL, false>(a, s, t, ok);
-    slot_values<P, ITEMS, FULL, false>(a, s, t, v);
+    slot_input_valid<P, ITEMS, FULL>(a, s, t, ok);
+    slot_values<P, ITEMS, FULL>(a, s, t, v);
     uint64_t *lacc = sacc + (size_t)s * (C + 2);
     uint64_t *gacc = a.tacc + (int64_t)s * stride;
     const int kind = m.slot_kind[s];
@@ -984,7 +956,7 @@ __global__ void __launch_bounds__(AGGS_THREADS) agg_update_smem_kernel(const __g
   const int tid = threadIdx.x & (AGG_THREADS - 1);
   const int64_t vb = (int64_t)blockIdx.x * AGGS_SUB + (threadIdx.x / AGG_THREADS), nvb = (int64_t)gridDim.x * AGGS_SUB;
   auto one_tile = [&](int64_t base) {
-    TileCtx t{nullptr, base + tid, a.n - 1};
+    TileCtx t{base + tid, a.n - 1};
     if (base + TILE <= a.n) process_tile_smem<P, ITEMS, true>(a, t, skeys, sacc, sctl, stride);
     else process_tile_smem<P, ITEMS, false>(a, t, skeys, sacc, sctl, stride);
   };
@@ -1021,71 +993,6 @@ __global__ void __launch_bounds__(AGGS_THREADS) agg_update_smem_kernel(const __g
     if (slot < 0) continue;
     for (int s = 0; s < ns; s++) global_op(m.slot_kind[s], &a.tacc[(int64_t)s * stride + slot], sacc[(size_t)s * (C + 2) + h]);
   }
-}
-
-// ---- staged kernel: TMA bulk copies + mbarrier pipeline ----------------------------------------------------------------
-// Every block owns the full tiles blockIdx.x, blockIdx.x + gridDim.x, ...  One elected thread asks the TMA engine to copy
-// the tile of every DISTINCT referenced buffer (each column once, however many expressions use it; validity bitmaps and
-// the materialised predicate too) into a shared-memory stage and arms the stage's mbarrier with the byte count; the
-// compute threads wait on the barrier's phase, consume the stage through shared-memory loads and hand it back with
-// __syncthreads().  nstages tiles are in flight per block, so HBM latency is hidden by the copy engine instead of by
-// occupancy and the compute warps never issue a global load.  The ragged tail is done by block 0 through the direct path.
-__device__ __forceinline__ void stage_issue(const AggArgs &a, int64_t tile, uint8_t *stage, uint64_t *bar) {
-  uint32_t total = 0;
-  for (int i = 0; i < a.nstaged; i++) total += (uint32_t)a.staged[i].bytes_per_tile;
-  mbar_arrive_expect_tx(bar, total);
-  for (int i = 0; i < a.nstaged; i++)
-    tma_load_1d(stage + a.staged[i].soff, a.staged[i].base + tile * (int64_t)a.staged[i].bytes_per_tile,
-                (uint32_t)a.staged[i].bytes_per_tile, bar);
-}
-
-template <class P, int ITEMS>
-__global__ void __launch_bounds__(AGG_THREADS) agg_update_staged_kernel(const __grid_constant__ AggArgs a) {
-  extern __shared__ __align__(128) uint8_t sm_staged[];
-  // layout: [stage 0 .. stage S-1][mbarriers (64 B)][dict_keys][acc]
-  constexpr int64_t TILE = (int64_t)AGG_THREADS * ITEMS;
-  const int S = a.nstages;
-  uint8_t *stages = sm_staged;
-  uint64_t *bars = (uint64_t *)(sm_staged + (size_t)S * a.stage_bytes);
-  uint64_t *dict_keys = bars + 8;
-  uint64_t *acc = dict_keys + AGG_DICT + 1;
-  const int tid = threadIdx.x;
-  const int64_t stride = a.cap + 2;
-  const int64_t full_tiles = a.n / TILE;
-  if (tid == 0) {
-    for (int i = 0; i < S; i++) mbar_init(&bars[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  dict_init<P>(a, dict_keys, acc, tid);
-  __syncthreads();
-  if (tid == 0) {   // prologue: fill the pipeline
-    for (int i = 0; i < S; i++) {
-      int64_t tile = (int64_t)blockIdx.x + (int64_t)i * gridDim.x;
-      if (tile < full_tiles) stage_issue(a, tile, stages + (size_t)i * a.stage_bytes, &bars[i]);
-    }
-  }
-  int64_t it = 0;
-  for (int64_t tile = blockIdx.x; tile < full_tiles; tile += gridDim.x, it++) {
-    const int st = (int)(it % S);
-    const uint32_t parity = (uint32_t)((it / S) & 1);
-    mbar_wait(&bars[st], parity);
-    if (!*(volatile int32_t *)a.flags) {
-      TileCtx t{stages + (size_t)st * a.stage_bytes, tid, TILE - 1};
-      process_tile<P, ITEMS, true, true>(a, t, dict_keys, acc, tid, stride);
-    }
-    __syncthreads();   // everyone is done reading this stage
-    if (tid == 0) {
-      int64_t next = tile + (int64_t)S * gridDim.x;
-      if (next < full_tiles) stage_issue(a, next, stages + (size_t)st * a.stage_bytes, &bars[st]);
-    }
-  }
-  if (blockIdx.x == 0 && full_tiles * TILE < a.n) {   // ragged tail through the direct path
-    TileCtx t{nullptr, full_tiles * TILE + tid, a.n - 1};
-    process_tile<P, ITEMS, false, false>(a, t, dict_keys, acc, tid, stride);
-  }
-  __syncthreads();
-  dict_merge<P>(a, dict_keys, acc, tid, stride);
 }
 
 // ---- wide grouping keys (> 63 bits, e.g. Q3's (l_orderkey, o_orderdate, o_shippriority)) -----------------------------
@@ -1131,7 +1038,7 @@ __global__ void __launch_bounds__(AGG_THREADS) agg_update_wide_kernel(const __gr
   const int64_t stride = a.cap + 2;
   for (int64_t base = (int64_t)blockIdx.x * TILE; base < a.n; base += (int64_t)gridDim.x * TILE) {
     if (*(volatile int32_t *)a.flags) break;
-    TileCtx t{nullptr, base + tid, a.n - 1};
+    TileCtx t{base + tid, a.n - 1};
     bool keep[ITEMS];
     uint64_t key[ITEMS][NW];
 #pragma unroll
@@ -1142,19 +1049,19 @@ __global__ void __launch_bounds__(AGG_THREADS) agg_update_wide_kernel(const __gr
     }
     if (m.has_mask) {
       int64_t x[ITEMS];
-      load_batch_as_i64<ITEMS, false, true, uint8_t>(a.col[m.mask_col].data, t, x);
+      load_batch_as_i64<ITEMS, false, uint8_t>(a.col[m.mask_col].data, t, x);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) keep[k] = keep[k] && x[k] != 0;
     }
-    apply_filter_terms<P, ITEMS, false, false>(a, t, keep);
+    apply_filter_terms<P, ITEMS, false>(a, t, keep);
     for (int i = 0; i < m.nkeys; i++) {
       const int kt = m.key_type[i], bits = m.key_bits[i], shift = m.key_shift[i];
       const KeyExtra ke = a.key_extra[i];
       int64_t x[ITEMS];
       bool valid[ITEMS];
-      if (kt == SB_FLOAT64) load_batch_as_i64<ITEMS, false, true, int64_t>(a.col[m.key_col[i]].data, t, x);
-      else load_i64_batch<ITEMS, false, true>(a.col[m.key_col[i]].data, kt, t, x);
-      if (m.key_valid[i]) load_valid_batch<ITEMS, false, true>(a.col[m.key_col[i]].valid, t, valid);
+      if (kt == SB_FLOAT64) load_batch_as_i64<ITEMS, false, int64_t>(a.col[m.key_col[i]].data, t, x);
+      else load_i64_batch<ITEMS, false>(a.col[m.key_col[i]].data, kt, t, x);
+      if (m.key_valid[i]) load_valid_batch<ITEMS, false>(a.col[m.key_col[i]].valid, t, valid);
 #pragma unroll
       for (int k = 0; k < ITEMS; k++) {
         if (m.key_valid[i] && !valid[k]) {
@@ -1195,7 +1102,7 @@ __global__ void __launch_bounds__(AGG_THREADS) agg_update_wide_kernel(const __gr
       doff[k] = -1;
       dst[k] = keep[k] ? table_slot_wide<NW>(a, key[k]) : -1;
     }
-    accumulate_slots<P, ITEMS, false, false>(a, t, dst, doff, nullptr, stride);
+    accumulate_slots<P, ITEMS, false>(a, t, dst, doff, nullptr, stride);
   }
 }
 

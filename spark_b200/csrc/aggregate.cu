@@ -48,7 +48,6 @@ namespace sb {
 // and the resulting kernels are cached by the plan's bytes (process + disk) -- what whole-stage codegen + Janino do for the
 // reference's CPU path.  Nothing in this file knows the shape of any particular query.
 constexpr int ITEMS_DIRECT = 8;   // rows per thread per tile, direct path (1024-row tiles)
-constexpr int ITEMS_STAGED = 4;   // staged path (512-row tiles keep two blocks per SM resident)
 
 typedef const void *AggKernel;    // a __global__ symbol or a cudaKernel_t from a run-time compiled library
 template <class K>
@@ -59,7 +58,7 @@ static void launch_agg(AggKernel k, int grid, int threads, size_t smem, cudaStre
 }
 constexpr int ITEMS_SMEM = 4;     // shared-memory tier: 512 threads x 4 rows
 struct KernelChoice {
-  AggKernel direct, staged;           // plain dictionary kernel (8 entries) and its TMA variant
+  AggKernel direct;                   // plain dictionary kernel (8 entries)
   int items_direct;
   std::string name;
   AggKernel smem = kptr(agg_update_smem_kernel<DynPlan, ITEMS_SMEM>);
@@ -95,11 +94,11 @@ static std::string plan_source(const PlanMeta &m) {
 static std::string kernel_expr(int which, int items) {
   const std::string it = std::to_string(items);
   switch (which) {
-    case NEED_K1: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 1, false, 4>";     // watch and yield, 4 entries
-    case NEED_K2: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 2, false, 8>";     // take over, 8 entries
-    case NEED_K1W: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 1, false, 8>";    // watch and yield, 8 entries
-    case NEED_K2B: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 2, false, 32>";   // take over, 32 entries (hash probed)
-    case NEED_DIRECT: return "sb::agg_update_kernel<sb::RP, 8, true, 0, false, 8>";           // plain (caller knows: <= 8 groups)
+    case NEED_K1: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 1, 4>";     // watch and yield, 4 entries
+    case NEED_K2: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 2, 8>";     // take over, 8 entries
+    case NEED_K1W: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 1, 8>";    // watch and yield, 8 entries
+    case NEED_K2B: return "sb::agg_update_kernel<sb::RP, " + it + ", false, 2, 32>";   // take over, 32 entries (hash probed)
+    case NEED_DIRECT: return "sb::agg_update_kernel<sb::RP, 8, true, 0, 8>";           // plain (caller knows: <= 8 groups)
     default: return "sb::agg_update_smem_kernel<sb::RP, 4>";
   }
 }
@@ -181,11 +180,11 @@ static bool specialise(const PlanMeta &m, int64_t n, int need, KernelChoice &kc)
 }
 
 static KernelChoice choose_kernels(const PlanMeta &m, int64_t n, int need) {
-  KernelChoice kc{kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT>), kptr(agg_update_staged_kernel<DynPlan, ITEMS_STAGED>), ITEMS_DIRECT, "generic"};
-  kc.k1 = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_YIELD, false, 4>);
-  kc.k2 = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_TAKEOVER, false, 8>);
-  kc.k1_wide = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_YIELD, false, 8>);
-  kc.k2_big = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_TAKEOVER, false, 32>);
+  KernelChoice kc{kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT>), ITEMS_DIRECT, "generic"};
+  kc.k1 = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_YIELD, 4>);
+  kc.k2 = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_TAKEOVER, 8>);
+  kc.k1_wide = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_YIELD, 8>);
+  kc.k2_big = kptr(agg_update_kernel<DynPlan, ITEMS_DIRECT, false, AGG_MODE_TAKEOVER, 32>);
   kc.k1_dict = 4;
   kc.k1_items = ITEMS_DIRECT;
   specialise(m, n, need, kc);
@@ -790,7 +789,7 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
   int need = light_plan ? (NEED_K1W | (big_dict_ok ? NEED_K2B : 0) | NEED_SMEM) : (NEED_K1 | NEED_K2 | NEED_SMEM);
   if (config().agg_tier == 1 || (config().agg_tier == 0 && plan->expected_groups > 0 && plan->expected_groups <= AGG_DICT)) need = NEED_DIRECT;
   else if (config().agg_tier == 2 || (config().agg_tier == 0 && plan->expected_groups > AGG_DICT)) need = NEED_SMEM;
-  KernelChoice kc = choose_kernels(m, a.nwords == 1 && !config().agg_staged ? n : 0, need);   // wide-key / staged kernels are not specialised
+  KernelChoice kc = choose_kernels(m, a.nwords == 1 ? n : 0, need);   // wide-key kernels are not specialised
   const size_t smem_acc = (size_t)(AGG_DICT + 1 + (size_t)(AGG_DICT + 1) * ns * AGG_THREADS) * 8;   // dictionary + fill counter + accumulators
   SB_REQUIRE(smem_acc <= 200 * 1024, "aggregate needs %zu bytes of shared memory", smem_acc);
   SB_CUDA(cudaFuncSetAttribute(kc.direct, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_acc));
@@ -844,54 +843,6 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
   if (tier != 1) SB_CUDA(cudaFuncSetAttribute(kc.smem, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   a.scap = scap;
 
-  // ---- staged (TMA) path: lay out one shared-memory stage holding the tile of every distinct referenced buffer ----
-  const int64_t stile = (int64_t)AGG_THREADS * ITEMS_STAGED;
-  bool staged = a.nwords == 1 && n >= stile && config().agg_staged != 0;   // experiment, off by default
-  size_t smem_staged = 0;
-  int grid_staged = 0;
-  if (staged) {
-    a.nstaged = 0;
-    int cursor = 0;
-    auto stage_of = [&](const void *base, int bytes_per_tile) -> int {
-      if (!staged || !base) return 0;
-      for (int i = 0; i < a.nstaged; i++)
-        if (a.staged[i].base == (const uint8_t *)base) return a.staged[i].soff;
-      if (a.nstaged >= AGG_MAX_STAGED || ((uintptr_t)base & 15) != 0) {   // too many buffers / TMA needs 16-byte alignment
-        staged = false;
-        return 0;
-      }
-      StagedBuf &sb_ = a.staged[a.nstaged++];
-      sb_.base = (const uint8_t *)base;
-      sb_.bytes_per_tile = bytes_per_tile;
-      sb_.soff = cursor;
-      cursor += (bytes_per_tile + 127) / 128 * 128;
-      return sb_.soff;
-    };
-    for (int i = 0; i < m.ncols; i++) {
-      ColRef &c = a.col[i];
-      c.soff = c.data ? stage_of(c.data, (int)stile * type_width(m.col_type[i] ? m.col_type[i] : SB_INT8)) : 0;
-      c.svoff = c.valid ? stage_of(c.valid, (int)stile / 8) : -1;
-    }
-    if (staged && a.nstaged > 0) {
-      a.stage_bytes = cursor;
-      const size_t fixed = 64 + smem_acc;   // mbarriers + dictionary + accumulators
-      int best_blocks = 0, best_stages = 0;
-      for (int blocks = 2; blocks >= 1 && !best_blocks; blocks--)
-        for (int S = AGG_MAX_STAGES; S >= 2; S--) {
-          size_t need = (size_t)S * cursor + fixed;
-          if (need <= 227 * 1024 && blocks * (need + 1024) <= 228 * 1024) { best_blocks = blocks; best_stages = S; break; }
-        }
-      if (best_blocks) {
-        a.nstages = best_stages;
-        smem_staged = (size_t)best_stages * cursor + fixed;
-        int64_t full_tiles = n / stile;
-        int64_t g = (int64_t)rt().num_sms * best_blocks;
-        grid_staged = (int)(full_tiles < g ? full_tiles : g);
-        SB_CUDA(cudaFuncSetAttribute(kc.staged, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      } else staged = false;
-    } else staged = false;
-  }
-
   Scratch flags(32, st), progress((int64_t)grid_k1 * (AGG_THREADS / 32) * 4 + 16, st), progress2((int64_t)grid_k1 * (AGG_THREADS / 32) * 4 + 16, st);
   std::unique_ptr<Scratch> slot_ids_buf;
   int64_t ngroups = 0;
@@ -922,8 +873,7 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
     if (n > 0) {
       KernelTimer kt(final_mode ? "agg_update_final" : "agg_update", st);
       a.gate = 0;
-      if (a.nwords == 1 && staged) launch_agg(kc.staged, grid_staged, AGG_THREADS, smem_staged, st, a);
-      else if (a.nwords == 1 && tier == 1) launch_agg(kc.direct, grid, AGG_THREADS, smem_acc, st, a);
+      if (a.nwords == 1 && tier == 1) launch_agg(kc.direct, grid, AGG_THREADS, smem_acc, st, a);
       else if (a.nwords == 1 && tier == 2) launch_agg(kc.smem, grid_smem, AGGS_THREADS, smem_tab, st, a);
       else if (a.nwords == 1) {
         a.gate = 1;
@@ -970,7 +920,7 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
   }
   g_last_plan_name = kc.name;
   if (config().agg_verbose) fprintf(stderr, "[sb_hash_aggregate] n=%lld plan=%s path=%s tier=%s cap=%lld slots=%d scap=%d\n", (long long)n, kc.name.c_str(),
-                                        a.nwords > 1 ? "wide" : (staged ? "staged" : "direct"), tier == 0 ? "auto" : (tier == 1 ? "dict" : "smem"),
+                                        a.nwords > 1 ? "wide" : "direct", tier == 0 ? "auto" : (tier == 1 ? "dict" : "smem"),
                                         (long long)cap, ns, scap);
   Scratch &slot_ids = *slot_ids_buf;
   if (plan->nkeys == 0 && ngroups == 0) {

@@ -28,7 +28,6 @@ struct Config {
   int agg_rtc = 1;                  // 0 off, 1 compile on first use
   int64_t agg_rtc_min_rows = 1 << 20;   // inputs smaller than this run the generic kernels (latency, not bandwidth)
   int agg_tier = 0;                 // 0 auto, 1 dictionary only, 2 shared-memory table only (tests)
-  int agg_staged = 0;               // TMA-staged update kernel (experiment)
   int agg_verbose = 0;
   int expr_interpret_only = 0;
   int regroup_ldst = 0;             // load/store multisplit instead of the copy-engine one

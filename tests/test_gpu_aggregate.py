@@ -192,13 +192,13 @@ def test_filter_project_operator(gpu, stream):
     assert_tables_equal(got, want, ordered=True)
 
 
-@pytest.mark.parametrize("env", [{"agg_rtc_min_rows": 0}, {"agg_rtc": 0}, {"agg_staged": 1},
+@pytest.mark.parametrize("env", [{"agg_rtc_min_rows": 0}, {"agg_rtc": 0},
                                  {"agg_tier": 2, "agg_rtc_min_rows": 0}, {"agg_tier": 1, "agg_rtc_min_rows": 0}, {"agg_tier": 2, "agg_rtc": 0},
                                  {"agg_tier": 1, "agg_rtc": 0}],
-                         ids=["rtc-chain", "generic-chain", "generic-tma", "rtc-smem-tier", "rtc-dict-tier", "generic-smem-tier", "generic-dict-tier"])
+                         ids=["rtc-chain", "generic-chain", "rtc-smem-tier", "rtc-dict-tier", "generic-smem-tier", "generic-dict-tier"])
 def test_every_update_kernel_variant_matches_the_oracle(gpu, stream, env, sbconfig):
-    """The run-time specialised (NVRTC, StaticPlan), generic (DynPlan), direct-load and TMA-staged update kernels share one code
-    base; each variant must produce the oracle's Q1 answer, including a ragged last tile and a NULL-able variant of the plan."""
+    """The run-time specialised (NVRTC, StaticPlan) and generic (DynPlan) update kernels share one code base; each variant
+    must produce the oracle's Q1 answer, including a ragged last tile and a NULL-able variant of the plan."""
     from spark_b200 import tpch
     from spark_b200.columnar import ColumnarBatch
     from spark_b200.execution import HashAggregateExec, LocalTableScanExec
@@ -214,7 +214,7 @@ def test_every_update_kernel_variant_matches_the_oracle(gpu, stream, env, sbconf
         part = tpch.q1_partial_plan(LocalTableScanExec(batch), fused=True).executeColumnar(stream)
         part.close()
         assert capi.load().sb_hash_aggregate_last_plan().decode().startswith("rtc:"), capi.load().sb_hash_aggregate_last_plan()
-    # same shape with NULLs in a key, an input and the filter column -> never matches a static table, exercises validity staging
+    # same shape with NULLs in a key, an input and the filter column -> never matches a static table, exercises the validity loads
     rng = np.random.default_rng(3)
     n = t.num_rows
     t2 = t.set_column(0, "l_quantity", pa.array(np.asarray(t.column("l_quantity")), mask=rng.random(n) < 0.1))
