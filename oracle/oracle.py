@@ -847,14 +847,9 @@ def _norm_key(v):
     return v
 
 
-def window(table, partition_cols, orders, specs):
-    """WindowExec (sql/core/.../window/WindowExec.scala:90-110 + WindowEvaluatorFactoryBase + WindowFunctionFrame.scala), one
-    partition at a time, the way the reference's frame classes walk it: growing frames accumulate as their upper bound moves,
-    shrinking frames are accumulated from the partition's end, sliding frames are re-evaluated over their rows.
-    orders: [(col, ascending, nulls_first)]; specs: [(func, col, (kind, lower, upper) | None, param, out_name)] with kind 'rows' |
-    'range', None bound = UNBOUNDED, 0 = CURRENT ROW, negative = PRECEDING (rows).  Default frame
-    (SpecifiedWindowFrame.defaultWindowFrame, windowExpressions.scala): RANGE UNBOUNDED PRECEDING..CURRENT ROW with an ORDER BY,
-    the whole partition without.  Output: rows sorted by partition keys (ASC NULLS FIRST) ++ orders, plus one column per spec."""
+def _window_layout(table, partition_cols, orders):
+    """The sorted input of a WindowExec and, per sorted row, its partition [seg_start, seg_end) and peer group
+    [peer_start, peer_end), plus the single ORDER BY key's values for RANGE frames with value offsets (None otherwise)."""
     key_cols = list(partition_cols) + [o[0] for o in orders]
     str_cols = [c for c in dict.fromkeys(key_cols) if pa.types.is_string(table.column(c).type) or pa.types.is_binary(table.column(c).type)]
     enc, _ = encode_string_columns(table, str_cols) if str_cols else (table, {})
@@ -880,9 +875,85 @@ def window(table, partition_cols, orders, specs):
                 seg_start[r], seg_end[r], peer_start[r], peer_end[r] = i, j, a, b
             a = b
         i = j
+    okey_vals = None
+    if len(orders) == 1:
+        okey_vals = srt.column(orders[0][0]).to_pylist()
+        if okey_vals and not isinstance(next((v for v in okey_vals if v is not None), 0), (int, float)):
+            okey_vals = [None if v is None else (v.toordinal() - 719163) for v in okey_vals] if pa.types.is_date(srt.column(orders[0][0]).type) else None
+    return srt, seg_start, seg_end, peer_start, peer_end, okey_vals
+
+
+def _frame_bounds(frame, orders, okey_vals, s, e, peer_start, peer_end, r):
+    """[lo, hi] (sorted rows, empty when lo > hi) of row r's frame in the partition [s, e)."""
+    kind, lower, upper = frame
+    if kind != "range":
+        return (s if lower is None else max(s, r + lower)), (e - 1 if upper is None else min(e - 1, r + upper))
+    # RANGE: UNBOUNDED -> partition end, CURRENT ROW (0) -> peer group end, else a VALUE offset over the single ORDER BY key:
+    # bound = key + offset for ASC, key - offset for DESC (WindowEvaluatorFactoryBase.createBoundOrdering); the frame is
+    # the rows whose keys lie between the bounds in the sort order; a NULL key has only its peers (RangeBoundOrdering)
+    ov = okey_vals[r] if okey_vals is not None else None
+    asc, nf = (orders[0][1], orders[0][2]) if orders else (True, True)
+
+    def side(q, bound):     # -1 the key of row q sorts before the bound, 0 equal, +1 after
+        k = okey_vals[q]
+        if k is None:
+            return -1 if nf else 1
+        c = int(_dcmp(float(k), float(bound))) if isinstance(k, float) or isinstance(bound, float) else (k > bound) - (k < bound)
+        return c if asc else -c
+
+    def first(pred):        # first position in [s, e) where pred holds (pred is monotone over the sorted partition)
+        a, b = s, e
+        while a < b:
+            m = (a + b) // 2
+            if pred(m):
+                b = m
+            else:
+                a = m + 1
+        return a
+
+    if lower is None:
+        lo = s
+    elif lower == 0 or ov is None:
+        lo = peer_start[r]
+    else:
+        bl = ov + lower if asc else ov - lower
+        lo = first(lambda q: side(q, bl) >= 0)
+    if upper is None:
+        hi = e - 1
+    elif upper == 0 or ov is None:
+        hi = peer_end[r] - 1
+    else:
+        bu = ov + upper if asc else ov - upper
+        hi = first(lambda q: side(q, bu) > 0) - 1
+    return lo, hi
+
+
+def _default_frame(frame, orders):
+    """SpecifiedWindowFrame.defaultWindowFrame (windowExpressions.scala): RANGE UNBOUNDED PRECEDING..CURRENT ROW with an ORDER BY,
+    the whole partition without."""
+    if frame is not None:
+        return frame
+    return ("range", None, 0) if orders else ("rows", None, None)
+
+
+def window_frames(table, partition_cols, orders, spec):
+    """[(lo, hi)] of every output row of window(table, partition_cols, orders, [spec]), as positions in its sorted order (empty
+    frame when lo > hi).  spec is one of window()'s spec tuples; only its frame is read."""
+    _, seg_start, seg_end, peer_start, peer_end, okey_vals = _window_layout(table, partition_cols, orders)
+    frame = _default_frame(spec[2], orders)
+    return [_frame_bounds(frame, orders, okey_vals, seg_start[r], seg_end[r], peer_start, peer_end, r) for r in range(len(seg_start))]
+
+
+def window(table, partition_cols, orders, specs):
+    """WindowExec (sql/core/.../window/WindowExec.scala:90-110 + WindowEvaluatorFactoryBase + WindowFunctionFrame.scala), one
+    partition at a time, the way the reference's frame classes walk it: growing frames accumulate as their upper bound moves,
+    shrinking frames are accumulated from the partition's end, sliding frames are re-evaluated over their rows.
+    orders: [(col, ascending, nulls_first)]; specs: [(func, col, (kind, lower, upper) | None, param, out_name)] with kind 'rows' |
+    'range', None bound = UNBOUNDED, 0 = CURRENT ROW, negative = PRECEDING (rows).  Default frame: _default_frame.
+    Output: rows sorted by partition keys (ASC NULLS FIRST) ++ orders, plus one column per spec."""
+    srt, seg_start, seg_end, peer_start, peer_end, okey_vals = _window_layout(table, partition_cols, orders)
+    n = table.num_rows
     out = {name: srt.column(name) for name in srt.column_names}
-    import functools
-    fkey = functools.cmp_to_key(lambda x, y: int(_dcmp(x, y)))
     seg_bounds = []
     i = 0
     while i < n:
@@ -893,15 +964,9 @@ def window(table, partition_cols, orders, specs):
         c = int(_dcmp(y, x)) if isinstance(x, float) else (y > x) - (y < x)
         return c < 0 if func == "min" else c > 0
 
-    okey_vals = None
-    if len(orders) == 1:
-        okey_vals = srt.column(orders[0][0]).to_pylist()
-        if okey_vals and not isinstance(next((v for v in okey_vals if v is not None), 0), (int, float)):
-            okey_vals = [None if v is None else (v.toordinal() - 719163) for v in okey_vals] if pa.types.is_date(srt.column(orders[0][0]).type) else None
     for func, col, frame, param, name in specs:
         vals = srt.column(col).to_pylist() if col is not None else None
-        if frame is None:
-            frame = ("range", None, 0) if orders else ("rows", None, None)
+        frame = _default_frame(frame, orders)
         kind, lower, upper = frame
         res = [None] * n
         for s, e in seg_bounds:
@@ -939,46 +1004,7 @@ def window(table, partition_cols, orders, specs):
                 continue
 
             def bounds(r):
-                if kind != "range":
-                    return (s if lower is None else max(s, r + lower)), (e - 1 if upper is None else min(e - 1, r + upper))
-                # RANGE: UNBOUNDED -> partition end, CURRENT ROW (0) -> peer group end, else a VALUE offset over the single ORDER BY key:
-                # bound = key + offset for ASC, key - offset for DESC (WindowEvaluatorFactoryBase.createBoundOrdering); the frame is
-                # the rows whose keys lie between the bounds in the sort order; a NULL key has only its peers (RangeBoundOrdering)
-                ov = okey_vals[r] if okey_vals is not None else None
-                asc, nf = (orders[0][1], orders[0][2]) if orders else (True, True)
-
-                def side(q, bound):     # -1 the key of row q sorts before the bound, 0 equal, +1 after
-                    k = okey_vals[q]
-                    if k is None:
-                        return -1 if nf else 1
-                    c = int(_dcmp(float(k), float(bound))) if isinstance(k, float) or isinstance(bound, float) else (k > bound) - (k < bound)
-                    return c if asc else -c
-
-                def first(pred):        # first position in [s, e) where pred holds (pred is monotone over the sorted partition)
-                    a, b = s, e
-                    while a < b:
-                        m = (a + b) // 2
-                        if pred(m):
-                            b = m
-                        else:
-                            a = m + 1
-                    return a
-
-                if lower is None:
-                    lo = s
-                elif lower == 0 or ov is None:
-                    lo = peer_start[r]
-                else:
-                    bl = ov + lower if asc else ov - lower
-                    lo = first(lambda q: side(q, bl) >= 0)
-                if upper is None:
-                    hi = e - 1
-                elif upper == 0 or ov is None:
-                    hi = peer_end[r] - 1
-                else:
-                    bu = ov + upper if asc else ov - upper
-                    hi = first(lambda q: side(q, bu) > 0) - 1
-                return lo, hi
+                return _frame_bounds(frame, orders, okey_vals, s, e, peer_start, peer_end, r)
 
             if func in ("first_value", "last_value"):
                 for r in range(s, e):

@@ -10,12 +10,16 @@
 //   3. heads -> dense ids (prefix sums) -> first row of every partition / peer group (scatter), so each row knows
 //      [seg_start, seg_end) and [peer_start, peer_end);
 //   4. every function is a per-row formula over those bounds and over SEGMENTED inclusive scans of its input (sum / count /
-//      min / max restart at partition heads): a frame [lo, hi] of a row is turned into S[hi] - S[lo - 1] (sum, count, avg) or
-//      M[hi] (min / max of frames that start at the partition's first row), first / last values and lag / lead are gathers.
+//      min / max restart at partition heads): a frame [lo, hi] of a row is turned into S[hi] - S[lo - 1] (count, integer sum),
+//      +0.0 + S[hi] (double sum / avg of a frame that starts at the partition's first row), +0.0 + the aligned block sums inside
+//      [lo, hi] (any other double sum / avg: the result depends on the frame's own rows only, so an inf, NaN or 1e20 before the
+//      frame cannot leak in), or M[hi] (min / max of frames that start at the partition's first row); first / last values and
+//      lag / lead are gathers.
 // Frames: ROWS with any bounds; RANGE with UNBOUNDED / CURRENT ROW bounds (the default frames) and with value offsets over one
 // numeric / date ORDER BY key (per-row binary searches in the sorted partition); min / max need a frame that starts at UNBOUNDED
 // PRECEDING.
 #include <memory>
+#include <type_traits>
 #include <vector>
 #include "common.cuh"
 #include "primitives.cuh"
@@ -319,10 +323,36 @@ __global__ void pick_kernel(Bounds b, int func, int frame_type, int64_t lower, i
   }
   idx[i] = j;
 }
-// sum / count / avg over the frame from the segmented prefixes (S = running sum of the non-NULL inputs, C = running count)
+// Block sums of the widened double inputs (NULL = 0.0): level j holds the sums of the aligned 2^j-row blocks, level 0 is the
+// input itself.  A double frame that does not start at its partition's first row is summed from the blocks that lie inside it,
+// so inf / NaN / large values outside the frame cannot reach its result (a difference of running sums would let them).
+constexpr int WIN_MAX_LEVELS = 32;
+struct BlockSums {
+  const double *level[WIN_MAX_LEVELS];
+};
+__global__ void block_sum_level_kernel(const double *__restrict__ below, int64_t m, double *__restrict__ out) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < m) out[k] = below[2 * k] + below[2 * k + 1];
+}
+// +0.0 (Spark's sums start from zero: Sum.scala coalesce(sum, 0) + x) plus, left to right, the largest aligned blocks that tile
+// [lo, hi]: at most 2 log2(hi - lo + 1) of them
+__device__ __forceinline__ double frame_block_sum(const BlockSums &bs, int64_t lo, int64_t hi) {
+  double acc = 0.0;
+  while (lo <= hi) {
+    int j = 63 - __clzll((unsigned long long)(hi - lo + 1));   // the widest block that fits ...
+    if (lo != 0 && __ffsll(lo) - 1 < j) j = __ffsll(lo) - 1;   // ... and is aligned at lo
+    acc = acc + bs.level[j][lo >> j];
+    lo += 1ll << j;
+  }
+  return acc;
+}
+
+// sum / count / avg over the frame.  C = running count; S = running sum of the non-NULL inputs.  Integers take S[hi] - S[lo - 1]
+// (exact modulo 2^64, like Spark's wrapping long sum).  Doubles take +0.0 + S[hi] when the frame starts at the partition's first
+// row and the block sums (bs) otherwise.
 template <typename T>
 __global__ void frame_sum_kernel(Bounds b, int func, int frame_type, int64_t lower, int64_t upper, const T *__restrict__ S, const int64_t *__restrict__ C,
-                                 void *__restrict__ out, uint32_t *__restrict__ out_valid) {
+                                 BlockSums bs, void *__restrict__ out, uint32_t *__restrict__ out_valid) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const bool in = i < b.n;
   bool valid = false;
@@ -336,8 +366,13 @@ __global__ void frame_sum_kernel(Bounds b, int func, int frame_type, int64_t low
       sum = S ? S[hi] : (T)0;
       cnt = C[hi];
       if (lo > s) {
-        if (S) sum -= S[lo - 1];
+        if (S) {
+          if constexpr (std::is_same<T, double>::value) sum = frame_block_sum(bs, lo, hi);
+          else sum -= S[lo - 1];
+        }
         cnt -= C[lo - 1];
+      } else if constexpr (std::is_same<T, double>::value) {
+        sum = sum + 0.0;   // a lone -0.0 sums to +0.0
       }
     }
     if (func == SB_WIN_COUNT) {
@@ -573,15 +608,30 @@ extern "C" int sb_window(const sb_table *in, const int32_t *partition_cols, int3
               vals = vavg.as<double>();
             }
             seg_scan<double, SEG_SUM>(vals, has.as<uint8_t>(), seg_head.as<int32_t>(), n, S.as<double>(), S_has.as<uint8_t>(), st);
-            frame_sum_kernel<double><<<wblocks(n), 256, 0, st>>>(b, w.func, w.frame_type, w.lower, w.upper, S.as<double>(), Cn.as<int64_t>(), c.data->ptr,
-                                                                 c.validity ? (uint32_t *)c.validity->ptr : nullptr);
+            // block sums for frames that may start after the partition's first row (about n more doubles)
+            BlockSums bs{};
+            bs.level[0] = vals;
+            Scratch blocks(w.lower != SB_UNBOUNDED_PRECEDING ? n * 8 + 16 : 0, st);
+            if (w.lower != SB_UNBOUNDED_PRECEDING) {
+              double *next = blocks.as<double>();
+              for (int j = 1; (n >> j) > 0; j++) {
+                const int64_t m = n >> j;
+                block_sum_level_kernel<<<wblocks(m), 256, 0, st>>>(bs.level[j - 1], m, next);
+                SB_LAUNCH_CHECK();
+                bs.level[j] = next;
+                next += m;
+              }
+            }
+            frame_sum_kernel<double><<<wblocks(n), 256, 0, st>>>(b, w.func, w.frame_type, w.lower, w.upper, S.as<double>(), Cn.as<int64_t>(), bs,
+                                                                 c.data->ptr, c.validity ? (uint32_t *)c.validity->ptr : nullptr);
           } else {
             seg_scan<int64_t, SEG_SUM>(vi.as<int64_t>(), has.as<uint8_t>(), seg_head.as<int32_t>(), n, S.as<int64_t>(), S_has.as<uint8_t>(), st);
-            frame_sum_kernel<int64_t><<<wblocks(n), 256, 0, st>>>(b, w.func, w.frame_type, w.lower, w.upper, S.as<int64_t>(), Cn.as<int64_t>(), c.data->ptr,
-                                                                  c.validity ? (uint32_t *)c.validity->ptr : nullptr);
+            frame_sum_kernel<int64_t><<<wblocks(n), 256, 0, st>>>(b, w.func, w.frame_type, w.lower, w.upper, S.as<int64_t>(), Cn.as<int64_t>(), BlockSums{},
+                                                                  c.data->ptr, c.validity ? (uint32_t *)c.validity->ptr : nullptr);
           }
         } else {
-          frame_sum_kernel<int64_t><<<wblocks(n), 256, 0, st>>>(b, w.func, w.frame_type, w.lower, w.upper, nullptr, Cn.as<int64_t>(), c.data->ptr, nullptr);
+          frame_sum_kernel<int64_t><<<wblocks(n), 256, 0, st>>>(b, w.func, w.frame_type, w.lower, w.upper, nullptr, Cn.as<int64_t>(), BlockSums{},
+                                                                c.data->ptr, nullptr);
         }
         SB_LAUNCH_CHECK();
       }
