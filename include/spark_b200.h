@@ -240,6 +240,22 @@ int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *dictionary, i
 #define SB_OP_CAST_F64 40
 #define SB_OP_CAST_I64 41
 #define SB_OP_CAST_I32 42
+/* string tests (UTF8_BINARY: unsigned bytes, UTF8String.binaryCompare).  Leaves: the string column is `arg` (never a COL node: a
+ * string COL is only valid as a bare one-node reference), the literal is the slice lit.i = offset << 32 | length of sb_expr.bytes.
+ * A NULL string gives NULL.  Comparisons have the column on the left ('x' < s is s > 'x'; s <> 'x' is NOT(STR_EQ)). */
+#define SB_OP_STR_EQ 50
+#define SB_OP_STR_LT 51
+#define SB_OP_STR_LE 52
+#define SB_OP_STR_GT 53
+#define SB_OP_STR_GE 54
+#define SB_OP_STR_IN 55            /* slice = uint32 count, then count records [uint32 length][bytes]; arg2 = 1: the list holds NULL
+                                      (no match -> NULL instead of FALSE, predicates.scala In / InSet) */
+#define SB_OP_STR_STARTS_WITH 56
+#define SB_OP_STR_ENDS_WITH 57
+#define SB_OP_STR_CONTAINS 58
+#define SB_OP_STR_LIKE 59          /* slice = the pattern (UTF-8); arg2 = the escape character (a code point <= 0xFFFF, usually '\\').
+                                      `_` matches one code point, `%` any run of them, newlines included */
+#define SB_OP_STR_OCTET_LENGTH 60  /* I32: the byte length; the slice is empty */
 
 /* value class of a node's result */
 #define SB_VT_BOOL 1
@@ -250,8 +266,8 @@ int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *dictionary, i
 typedef struct sb_expr_node {
   int32_t op;       /* SB_OP_* */
   int32_t vtype;    /* SB_VT_* of the result */
-  int32_t arg;      /* SB_OP_COL: column index */
-  int32_t pad;
+  int32_t arg;      /* SB_OP_COL, SB_OP_STR_*: column index; comparisons: operand class; CAST: source class */
+  int32_t arg2;     /* SB_OP_STR_LIKE: escape code point; SB_OP_STR_IN: 1 = the list holds NULL; 0 everywhere else */
   union { int64_t i; double d; } lit;
 } sb_expr_node;
 
@@ -259,6 +275,8 @@ typedef struct sb_expr {
   const sb_expr_node *nodes;   /* postfix order */
   int32_t n;
   int32_t out_type;            /* SB_* type of the materialised result column */
+  const uint8_t *bytes;        /* host bytes of the literals of SB_OP_STR_* nodes (NULL when there are none) */
+  int64_t nbytes;
 } sb_expr;
 
 /* FilterExec + ProjectExec in one pass: rows where `predicate` is TRUE survive (NULL drops the row);

@@ -45,7 +45,7 @@ public final class Native {
 
   // ---- expressions, FilterExec / ProjectExec --------------------------------------------------------------------------------
   /** postfix sb_expr program built by ExprCompiler; returns a native handle freed with exprFree. */
-  public static native long exprCreate(int[] ops, int[] vtypes, int[] args, long[] literals, int outType);
+  public static native long exprCreate(int[] ops, int[] vtypes, int[] args, int[] args2, long[] literals, byte[] bytes, int outType);
   public static native void exprFree(long expr);
   public static native long filterProject(long table, long predicateExpr, long[] projectionExprs, long stream);
 

@@ -154,20 +154,28 @@ NATIVE(jlong, tableExportHost)(JNIEnv *env, jclass c, jlong table, jint column, 
   return (jlong)nulls;
 }
 
-NATIVE(jlong, exprCreate)(JNIEnv *env, jclass c, jintArray ops, jintArray vtypes, jintArray args, jlongArray literals, jint outType) {
+NATIVE(jlong, exprCreate)(JNIEnv *env, jclass c, jintArray ops, jintArray vtypes, jintArray args, jintArray args2, jlongArray literals,
+                          jbyteArray bytes, jint outType) {
   jsize n = (*env)->GetArrayLength(env, ops);
+  jsize nb = (*env)->GetArrayLength(env, bytes);
   jint *o = (*env)->GetIntArrayElements(env, ops, NULL), *v = (*env)->GetIntArrayElements(env, vtypes, NULL);
-  jint *a = (*env)->GetIntArrayElements(env, args, NULL);
+  jint *a = (*env)->GetIntArrayElements(env, args, NULL), *a2 = (*env)->GetIntArrayElements(env, args2, NULL);
   jlong *l = (*env)->GetLongArrayElements(env, literals, NULL);          /* doubles travel as their bit pattern */
-  sb_expr *e = (sb_expr *)malloc(sizeof(sb_expr));
+  sb_expr *e = (sb_expr *)calloc(1, sizeof(sb_expr));
   sb_expr_node *nodes = (sb_expr_node *)calloc((size_t)(n ? n : 1), sizeof(sb_expr_node));
   for (jsize i = 0; i < n; i++) {
-    nodes[i].op = o[i]; nodes[i].vtype = v[i]; nodes[i].arg = a[i]; nodes[i].lit.i = l[i];
+    nodes[i].op = o[i]; nodes[i].vtype = v[i]; nodes[i].arg = a[i]; nodes[i].arg2 = a2[i]; nodes[i].lit.i = l[i];
   }
   e->nodes = nodes; e->n = n; e->out_type = outType;
+  if (nb > 0) {                                                          /* the string literals' pool (SB_OP_STR_* slices) */
+    uint8_t *pool = (uint8_t *)malloc((size_t)nb);
+    (*env)->GetByteArrayRegion(env, bytes, 0, nb, (jbyte *)pool);
+    e->bytes = pool; e->nbytes = nb;
+  }
   (*env)->ReleaseIntArrayElements(env, ops, o, JNI_ABORT);
   (*env)->ReleaseIntArrayElements(env, vtypes, v, JNI_ABORT);
   (*env)->ReleaseIntArrayElements(env, args, a, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, args2, a2, JNI_ABORT);
   (*env)->ReleaseLongArrayElements(env, literals, l, JNI_ABORT);
   return (jlong)(intptr_t)e;
 }
@@ -176,6 +184,7 @@ NATIVE(void, exprFree)(JNIEnv *env, jclass c, jlong expr) {
   sb_expr *e = (sb_expr *)(intptr_t)expr;
   if (e) {
     free((void *)e->nodes);
+    free((void *)e->bytes);
     free(e);
   }
 }

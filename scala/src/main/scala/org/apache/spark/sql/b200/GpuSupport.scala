@@ -16,6 +16,7 @@ import org.apache.spark.sql.execution.joins.{BroadcastHashJoinExec, ShuffledHash
 import org.apache.spark.sql.internal.SQLConf
 import org.apache.spark.sql.types._
 import org.apache.spark.sql.vectorized.ColumnarBatch
+import org.apache.spark.unsafe.types.UTF8String
 
 /**
  * What the GPU path can run and how Catalyst objects become the POD structures of include/spark_b200.h.  Anything this object
@@ -314,9 +315,29 @@ object GpuSupport {
  * Kleene AND / OR, casts between the numeric classes.  `supported` is the single source of truth for what may be offloaded.
  */
 object ExprCompiler {
-  final case class Program(ops: Array[Int], vtypes: Array[Int], args: Array[Int], literals: Array[Long], outType: Int) {
-    def create(): Long = Native.exprCreate(ops, vtypes, args, literals, outType)
+  final case class Program(ops: Array[Int], vtypes: Array[Int], args: Array[Int], args2: Array[Int], literals: Array[Long], bytes: Array[Byte],
+                           outType: Int) {
+    def create(): Long = Native.exprCreate(ops, vtypes, args, args2, literals, bytes, outType)
   }
+  // String tests run on the GPU against foldable literals over a column of the UTF8_BINARY collation (byte order = Spark's order);
+  // they become SB_OP_STR_* leaves that name the column, the literal bytes travel in the program's pool.
+  private def binaryString(dt: DataType): Boolean = dt match {
+    case st: StringType => st.isUTF8BinaryCollation
+    case _ => false
+  }
+  private def strCol(e: Expression): Boolean = e match {
+    case a: AttributeReference => binaryString(a.dataType)
+    case _ => false
+  }
+  private def strLit(e: Expression): Boolean = e match {
+    case Literal(v, dt) => v != null && binaryString(dt)
+    case _ => false
+  }
+  private val strCmpOps: PartialFunction[Expression, Int] = {        // SB_OP_STR_EQ .. SB_OP_STR_GE
+    case _: EqualTo => 50; case _: LessThan => 51; case _: LessThanOrEqual => 52; case _: GreaterThan => 53; case _: GreaterThanOrEqual => 54
+  }
+  private def strCompare(b: BinaryComparison): Boolean =
+    strCmpOps.isDefinedAt(b) && ((strCol(b.left) && strLit(b.right)) || (strLit(b.left) && strCol(b.right)))
   private def vt(dt: DataType): Int = dt match {       // SB_VT_*
     case BooleanType => 1
     case ByteType | ShortType | IntegerType | DateType => 2
@@ -325,6 +346,14 @@ object ExprCompiler {
     case _ => -1
   }
   def supported(e: Expression): Boolean = e match {
+    case b: BinaryComparison if strCompare(b) => true
+    case In(c, list) if strCol(c) && list.forall(l => l.isInstanceOf[Literal] && binaryString(l.dataType)) => true
+    case InSet(c, _) if strCol(c) => true
+    case StartsWith(c, l) => strCol(c) && strLit(l)
+    case EndsWith(c, l) => strCol(c) && strLit(l)
+    case Contains(c, l) => strCol(c) && strLit(l)
+    case Like(c, l, _) => strCol(c) && strLit(l)
+    case OctetLength(c) => strCol(c)
     case a: AttributeReference => GpuExec.typeId(a.dataType) > 0
     case Alias(c, _) => supported(c)
     case l: Literal => vt(l.dataType) > 0        // a NULL literal too: LIT_NULL carries its class (an untyped NULL has none)
@@ -344,9 +373,33 @@ object ExprCompiler {
   }
   def compile(e: Expression, in: Seq[Attribute]): Program = {
     val ops = new ArrayBuffer[Int](); val vts = new ArrayBuffer[Int](); val args = new ArrayBuffer[Int](); val lits = new ArrayBuffer[Long]()
-    def emit(op: Int, v: Int, arg: Int = 0, lit: Long = 0L): Unit = { ops += op; vts += v; args += arg; lits += lit }
+    val args2 = new ArrayBuffer[Int](); val pool = new java.io.ByteArrayOutputStream()
+    def emit(op: Int, v: Int, arg: Int = 0, lit: Long = 0L, arg2: Int = 0): Unit = { ops += op; vts += v; args += arg; lits += lit; args2 += arg2 }
+    def slice(b: Array[Byte]): Long = { val off = pool.size().toLong; pool.write(b, 0, b.length); (off << 32) | b.length.toLong }
+    def colOf(c: Expression): Int = in.indexWhere(_.exprId == c.asInstanceOf[AttributeReference].exprId)
+    def bytesOf(l: Expression): Array[Byte] = l.asInstanceOf[Literal].value.asInstanceOf[UTF8String].getBytes
+    def strTest(op: Int, c: Expression, l: Expression, arg2: Int = 0): Unit = emit(op, 1, colOf(c), slice(bytesOf(l)), arg2)
+    def strIn(c: Expression, values: Seq[Any]): Unit = {                 // [count][length][bytes]... in the host's byte order
+      val present = values.filter(_ != null).map(_.asInstanceOf[UTF8String].getBytes)
+      val buf = java.nio.ByteBuffer.allocate(4 + present.map(4 + _.length).sum).order(java.nio.ByteOrder.nativeOrder())
+      buf.putInt(present.length)
+      present.foreach { b => buf.putInt(b.length); buf.put(b) }
+      emit(55, 1, colOf(c), slice(buf.array()), if (present.length != values.length) 1 else 0)
+    }
     def bin(op: Int, l: Expression, r: Expression, v: Int, arg: Int = 0): Unit = { go(l); go(r); emit(op, v, arg) }
     def go(x: Expression): Unit = x match {
+      case b: BinaryComparison if strCompare(b) =>                       // the column on the left: 'x' < s is s > 'x'
+        val flipped = strLit(b.left)
+        val op = strCmpOps(b)
+        val op2 = if (!flipped) op else op match { case 51 => 53; case 52 => 54; case 53 => 51; case 54 => 52; case o => o }
+        if (flipped) strTest(op2, b.right, b.left) else strTest(op2, b.left, b.right)
+      case In(c, list) if strCol(c) => strIn(c, list.map(_.asInstanceOf[Literal].value))
+      case InSet(c, hset) if strCol(c) => strIn(c, hset.toSeq)
+      case StartsWith(c, l) => strTest(56, c, l)
+      case EndsWith(c, l) => strTest(57, c, l)
+      case Contains(c, l) => strTest(58, c, l)
+      case Like(c, l, esc) => strTest(59, c, l, esc.toInt)
+      case OctetLength(c) => emit(60, 2, colOf(c))
       case a: AttributeReference => emit(1, vt(a.dataType), in.indexWhere(_.exprId == a.exprId))
       case Alias(c, _) => go(c)
       case Literal(null, dt) => emit(4, vt(dt))
@@ -373,6 +426,6 @@ object ExprCompiler {
       case other => throw new B200Exception(5, s"expression $other is not supported on the GPU path")
     }
     go(e)
-    Program(ops.toArray, vts.toArray, args.toArray, lits.toArray, GpuExec.typeId(e.dataType))
+    Program(ops.toArray, vts.toArray, args.toArray, args2.toArray, lits.toArray, pool.toByteArray, GpuExec.typeId(e.dataType))
   }
 }

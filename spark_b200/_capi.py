@@ -18,7 +18,9 @@ SB_OK = 0
 (SB_BOOL, SB_INT8, SB_INT16, SB_INT32, SB_INT64, SB_FLOAT32, SB_FLOAT64, SB_DATE32, SB_TIMESTAMP, SB_DECIMAL64,
  SB_STRING, SB_DECIMAL128) = range(1, 13)
 SB_OP = dict(COL=1, LIT_I64=2, LIT_F64=3, LIT_NULL=4, ADD=10, SUB=11, MUL=12, DIV=13, NEG=14, EQ=20, NE=21, LT=22,
-             LE=23, GT=24, GE=25, AND=30, OR=31, NOT=32, ISNULL=33, ISNOTNULL=34, CAST_F64=40, CAST_I64=41, CAST_I32=42)
+             LE=23, GT=24, GE=25, AND=30, OR=31, NOT=32, ISNULL=33, ISNOTNULL=34, CAST_F64=40, CAST_I64=41, CAST_I32=42,
+             STR_EQ=50, STR_LT=51, STR_LE=52, STR_GT=53, STR_GE=54, STR_IN=55, STR_STARTS_WITH=56, STR_ENDS_WITH=57, STR_CONTAINS=58,
+             STR_LIKE=59, STR_OCTET_LENGTH=60)
 SB_VT_BOOL, SB_VT_I32, SB_VT_I64, SB_VT_F64 = 1, 2, 3, 4
 SB_AGG = dict(sum=1, avg=2, count=3, count_star=4, min=5, max=6)
 SB_AGG_MODE = dict(partial=1, final=2, complete=3, partial_merge=4)
@@ -53,11 +55,11 @@ class _lit(C.Union):
 
 
 class sb_expr_node(C.Structure):
-    _fields_ = [("op", C.c_int32), ("vtype", C.c_int32), ("arg", C.c_int32), ("pad", C.c_int32), ("lit", _lit)]
+    _fields_ = [("op", C.c_int32), ("vtype", C.c_int32), ("arg", C.c_int32), ("arg2", C.c_int32), ("lit", _lit)]
 
 
 class sb_expr(C.Structure):
-    _fields_ = [("nodes", C.POINTER(sb_expr_node)), ("n", C.c_int32), ("out_type", C.c_int32)]
+    _fields_ = [("nodes", C.POINTER(sb_expr_node)), ("n", C.c_int32), ("out_type", C.c_int32), ("bytes", C.c_void_p), ("nbytes", C.c_int64)]
 
 
 class sb_agg_spec(C.Structure):

@@ -327,6 +327,8 @@ static int build_tree(const sb_expr &e, std::vector<ExprTree> &t) {
     nd.lit = e.nodes[i].lit.i;
     switch (nd.op) {
       case SB_OP_COL: case SB_OP_LIT_I64: case SB_OP_LIT_F64: case SB_OP_LIT_NULL: break;
+      case SB_OP_STR_EQ: case SB_OP_STR_LT: case SB_OP_STR_LE: case SB_OP_STR_GT: case SB_OP_STR_GE: case SB_OP_STR_IN:
+      case SB_OP_STR_STARTS_WITH: case SB_OP_STR_ENDS_WITH: case SB_OP_STR_CONTAINS: case SB_OP_STR_LIKE: case SB_OP_STR_OCTET_LENGTH: break;
       case SB_OP_NEG: case SB_OP_NOT: case SB_OP_ISNULL: case SB_OP_ISNOTNULL:
       case SB_OP_CAST_F64: case SB_OP_CAST_I64: case SB_OP_CAST_I32:
         nd.l = stack.back(); stack.pop_back(); break;
@@ -1068,8 +1070,10 @@ struct sb_agg_state {
   std::vector<int32_t> key_cols;
   std::vector<sb_agg_spec> aggs;
   std::vector<std::vector<sb_expr_node>> nodes;
+  std::vector<std::vector<uint8_t>> bytes;   // string literal pools of the inputs
   sb_expr filter;
   std::vector<sb_expr_node> filter_nodes;
+  std::vector<uint8_t> filter_bytes;
   std::vector<int32_t> merged_keys;       // 0..nkeys-1: where the keys sit in a Partial table
   std::vector<sb_table *> parked;
   int64_t parked_rows = 0;
@@ -1115,11 +1119,17 @@ extern "C" int sb_hash_agg_create(const sb_agg_plan *plan, sb_agg_state **out) {
   st->key_cols.assign(plan->key_cols, plan->key_cols + plan->nkeys);
   st->aggs.assign(plan->aggs, plan->aggs + plan->naggs);
   st->nodes.resize(plan->naggs);
+  st->bytes.resize(plan->naggs);
+  auto copy_pool = [](const sb_expr &e, std::vector<uint8_t> &to, sb_expr &copy) {
+    if (e.bytes && e.nbytes > 0) to.assign(e.bytes, e.bytes + e.nbytes);
+    copy.bytes = to.empty() ? nullptr : to.data();
+  };
   for (int i = 0; i < plan->naggs; i++) {
     const sb_expr &e = plan->aggs[i].input;
     if (e.nodes && e.n > 0) {
       st->nodes[i].assign(e.nodes, e.nodes + e.n);
       st->aggs[i].input.nodes = st->nodes[i].data();
+      copy_pool(e, st->bytes[i], st->aggs[i].input);
     } else {
       st->aggs[i].input.nodes = nullptr;
       st->aggs[i].input.n = 0;
@@ -1132,6 +1142,7 @@ extern "C" int sb_hash_agg_create(const sb_agg_plan *plan, sb_agg_state **out) {
     st->filter_nodes.assign(plan->filter->nodes, plan->filter->nodes + plan->filter->n);
     st->filter = *plan->filter;
     st->filter.nodes = st->filter_nodes.data();
+    copy_pool(*plan->filter, st->filter_bytes, st->filter);
     st->plan.filter = &st->filter;
   }
   for (int i = 0; i < plan->nkeys; i++) st->merged_keys.push_back(i);

@@ -11,6 +11,7 @@
 #include <vector>
 #include "expr.cuh"
 #include "simple_pred.cuh"
+#include "strpred.cuh"
 #include "primitives.cuh"
 #include "rtc.cuh"
 
@@ -19,8 +20,8 @@ namespace sb {
 constexpr int EXPR_MAX_COLS = 12;
 
 struct DevNode {
-  int32_t op, vtype, arg, pad;
-  int64_t lit;
+  int32_t op, vtype, arg, arg2;
+  int64_t lit;   // string tests: the descriptor's word index in `blob`
 };
 struct DevProg {
   int32_t n;
@@ -28,7 +29,9 @@ struct DevProg {
   DevNode nodes[EXPR_MAX_NODES];
   const void *col_data[EXPR_MAX_COLS];
   const uint8_t *col_valid[EXPR_MAX_COLS];
+  const int32_t *col_offsets[EXPR_MAX_COLS];   // string columns
   int32_t col_type[EXPR_MAX_COLS];
+  const uint32_t *blob;                        // the program's string literals (strpred.cuh), or null
 };
 
 static int vtype_of_column(int32_t t) {
@@ -141,7 +144,17 @@ void expr_validate(const sb_table *in, const sb_expr &e) {
         depth--;
         break;
       }
-      default: fail(SB_ERR_INVALID, "unknown expression op %d at node %d", nd.op, i);
+      default: {
+        if (!strpred_is_leaf(nd.op)) fail(SB_ERR_INVALID, "unknown expression op %d at node %d", nd.op, i);
+        res = strpred_validate(in, e, i);
+        bool seen = false;
+        for (int c = 0; c < ncols; c++) seen |= cols_seen[c] == nd.arg;
+        if (!seen) {
+          SB_REQUIRE(ncols < EXPR_MAX_COLS, "expression references more than %d distinct columns", EXPR_MAX_COLS);
+          cols_seen[ncols++] = nd.arg;
+        }
+        break;
+      }
     }
     SB_REQUIRE(depth < EXPR_STACK, "expression needs more than %d stack slots", EXPR_STACK);
     vt[depth] = res;
@@ -154,17 +167,19 @@ void expr_validate(const sb_table *in, const sb_expr &e) {
 bool expr_nullable(const sb_table *in, const sb_expr &e) {
   for (int i = 0; i < e.n; i++) {
     const sb_expr_node &nd = e.nodes[i];
-    if (nd.op == SB_OP_COL && in->cols[nd.arg].validity) return true;
+    if ((nd.op == SB_OP_COL || strpred_is_leaf(nd.op)) && in->cols[nd.arg].validity) return true;
+    if (nd.op == SB_OP_STR_IN && nd.arg2) return true;
     if (nd.op == SB_OP_DIV || nd.op == SB_OP_LIT_NULL) return true;
   }
   return false;
 }
 
-// `e` has passed expr_validate
-static DevProg build_prog(const sb_table *in, const sb_expr &e) {
+// `e` has passed expr_validate; `tests` / `blob` are its string literals (strpred_compile) and their device copy
+static DevProg build_prog(const sb_table *in, const sb_expr &e, const StrTests &tests, const uint32_t *blob) {
   DevProg p;
   p.n = e.n;
   p.ncols = 0;
+  p.blob = blob;
   int remap[256];
   for (int i = 0; i < 256; i++) remap[i] = -1;
   for (int i = 0; i < e.n; i++) {
@@ -172,15 +187,16 @@ static DevProg build_prog(const sb_table *in, const sb_expr &e) {
     p.nodes[i].op = nd.op;
     p.nodes[i].vtype = nd.vtype;
     p.nodes[i].arg = nd.arg;
-    p.nodes[i].pad = 0;
-    p.nodes[i].lit = nd.lit.i;
-    if (nd.op == SB_OP_COL) {
+    p.nodes[i].arg2 = nd.arg2;
+    p.nodes[i].lit = strpred_is_leaf(nd.op) ? (int64_t)tests.ref[i] : nd.lit.i;
+    if (nd.op == SB_OP_COL || strpred_is_leaf(nd.op)) {
       SB_REQUIRE(nd.arg < 256, "expression column index too large");
       if (remap[nd.arg] < 0) {
         SB_REQUIRE(p.ncols < EXPR_MAX_COLS, "expression references more than %d distinct columns", EXPR_MAX_COLS);
         const Column &c = in->cols[nd.arg];
         p.col_data[p.ncols] = c.d();
         p.col_valid[p.ncols] = c.v();
+        p.col_offsets[p.ncols] = c.o();
         p.col_type[p.ncols] = c.type;
         remap[nd.arg] = p.ncols++;
       }
@@ -196,6 +212,11 @@ __device__ __forceinline__ int cmp_f64(double x, double y) {
   bool xn = x != x, yn = y != y;
   if (xn || yn) return (int)xn - (int)yn;
   return x < y ? -1 : 1;
+}
+
+// the string tests out of line: inlined, they push eval_row's projection kernel into spilling
+__device__ __noinline__ int64_t eval_string_test(int32_t op, uint32_t ref, const uint32_t *blob, const uint8_t *s, int32_t n) {
+  return strpred_eval(op, ref, blob, s, n);
 }
 
 // evaluates the program for one row; returns raw 64-bit value and null flag
@@ -293,6 +314,18 @@ __device__ __forceinline__ void eval_row(const DevProg &p, int64_t row, int64_t 
           st[sp - 1] = d != d ? 0 : (int64_t)__double2int_rz(d);
         } else st[sp - 1] = (int64_t)(int32_t)(uint32_t)st[sp - 1];
         break;
+      case SB_OP_STR_EQ: case SB_OP_STR_LT: case SB_OP_STR_LE: case SB_OP_STR_GT: case SB_OP_STR_GE: case SB_OP_STR_IN:
+      case SB_OP_STR_STARTS_WITH: case SB_OP_STR_ENDS_WITH: case SB_OP_STR_CONTAINS: case SB_OP_STR_LIKE: case SB_OP_STR_OCTET_LENGTH: {
+        const int c = nd.arg;
+        const bool v = bit_valid(p.col_valid[c], row);
+        int64_t x = 0;
+        if (v) {
+          const int32_t b = p.col_offsets[c][row];
+          x = eval_string_test(nd.op, (uint32_t)nd.lit, p.blob, (const uint8_t *)p.col_data[c] + b, p.col_offsets[c][row + 1] - b);
+        }
+        st[sp] = x; nl[sp] = !v || (nd.op == SB_OP_STR_IN && x == 0 && nd.arg2 != 0); sp++;
+        break;
+      }
     }
   }
   out = st[0];
@@ -422,7 +455,9 @@ void eval_predicate(const sb_table *in, const sb_expr &pred, uint8_t *mask, cuda
     SB_LAUNCH_CHECK();
     return;
   }
-  DevProg p = build_prog(in, pred);
+  const StrTests tests = strpred_compile(pred);
+  StrBlob blob(tests, st);
+  DevProg p = build_prog(in, pred, tests, blob.ptr());
   predicate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, n, mask);
   SB_LAUNCH_CHECK();
 }
@@ -435,7 +470,9 @@ Column eval_projection(const sb_table *in, const sb_expr &e, const int64_t *sel,
     return gather_column(in->cols[col], sel, nout, false, st);
   }
   expr_validate(in, e);
-  DevProg p = build_prog(in, e);
+  const StrTests tests = strpred_compile(e);
+  StrBlob blob(tests, st);
+  DevProg p = build_prog(in, e, tests, blob.ptr());
   SB_REQUIRE(e.out_type != SB_STRING && type_width(e.out_type) > 0, "bad projection result type %d", e.out_type);
   Column r = column_alloc(e.out_type, 0, nout, expr_nullable(in, e), st);
   if (nout == 0) return r;

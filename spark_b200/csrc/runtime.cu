@@ -361,7 +361,7 @@ int sb_table_import_host(const sb_column *cols, int32_t ncols, sb_stream *s, sb_
           SB_CUDA(cudaMemsetAsync(c.offsets->ptr, 0, 4, st));
         }
         c.string_bytes = last;
-        c.data = buffer_alloc(last + 16, st);
+        c.data = buffer_alloc((int64_t)last + 16, st);   // an arena of up to 2^31 - 1 bytes: the padding must not wrap int32
         if (last > 0) SB_CUDA(cudaMemcpyAsync(c.data->ptr, h.data, (size_t)last, cudaMemcpyHostToDevice, st));
       } else {
         int w = type_width(h.type);

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import datetime
+import struct
 
 from . import _capi as capi
 
@@ -78,11 +79,12 @@ def _wrap(x):
     return x if isinstance(x, Expression) else Literal(x)
 
 
-def _node(op, vtype, arg=0, lit_i=None, lit_d=None):
+def _node(op, vtype, arg=0, lit_i=None, lit_d=None, arg2=0):
     n = capi.sb_expr_node()
     n.op = capi.SB_OP[op]
     n.vtype = vtype
     n.arg = arg
+    n.arg2 = arg2
     if lit_d is not None:
         n.lit.d = lit_d
     elif lit_i is not None:
@@ -120,7 +122,9 @@ class Literal(Expression):
             vt = vt or VT_I32
         self.value = value
         if vt is None:
-            if value is None:
+            if isinstance(value, (str, bytes)):
+                vt = 0                       # a string: only the string tests below take one
+            elif value is None:
                 vt = VT_I64
             elif isinstance(value, bool):
                 vt = VT_BOOL
@@ -134,6 +138,8 @@ class Literal(Expression):
         return self.vt
 
     def emit(self, schema, out):
+        if self.vt == 0:
+            raise TypeError("a string literal is only an operand of a string test (comparison, IN, LIKE, StartsWith ...)")
         if self.value is None:
             out.append(_node("LIT_NULL", self.vt))
         elif self.vt == VT_F64:
@@ -143,6 +149,8 @@ class Literal(Expression):
 
     def sexpr(self):
         import numpy as np
+        if self.vt == 0:
+            return ("lit", self.value, type(self.value))
         dt = {VT_BOOL: bool, VT_I32: np.int32, VT_I64: np.int64, VT_F64: np.float64}[self.vt]
         return ("lit", self.value, dt)
 
@@ -259,13 +267,30 @@ class _Comparison(Expression):
     def vtype(self, schema):
         return VT_BOOL
 
+    def _string_sides(self):
+        """(column, literal bytes, flipped) when this compares a string column with a string literal, else None."""
+        l, r = self.left, self.right
+        if isinstance(r, AttributeReference) and _is_str_lit(l):
+            return r, _utf8(l.value), True
+        if isinstance(l, AttributeReference) and _is_str_lit(r):
+            return l, _utf8(r.value), False
+        return None
+
     def emit(self, schema, out):
+        s = self._string_sides()
+        if s is not None:                            # STR_* keeps the column on the left: 'x' < s is s > 'x'
+            c, b, flipped = s
+            op = _FLIP[self.op] if flipped else self.op
+            out.append(_node("STR_" + op, VT_BOOL, _string_col(c, schema), lit_i=_pool(out).slice(b)))
+            return
         vt = _promote(self.left.vtype(schema), self.right.vtype(schema))
         _coerce(self.left, schema, vt).emit(schema, out)
         _coerce(self.right, schema, vt).emit(schema, out)
         out.append(_node(self.op, VT_BOOL, vt))   # arg = operand class
 
     def sexpr(self):
+        if self._string_sides() is not None:
+            return ("str_cmp", self.name, self.left.sexpr(), self.right.sexpr())
         return (self.name, self.left.sexpr(), self.right.sexpr())
 
 
@@ -348,16 +373,142 @@ class IsNotNull(_Unary):
     op, name = "ISNOTNULL", "isnotnull"
 
 
+# ---- string tests against literals (stringExpressions.scala, regexpExpressions.scala Like, predicates.scala In / InSet) --------
+# Each lowers to one SB_OP_STR_* leaf naming its column; the literal bytes go to the program's pool (include/spark_b200.h).
+class _Program(list):
+    """The node list an expression emits into, with the pool its string literals are appended to."""
+
+    def __init__(self):
+        super().__init__()
+        self.pool = bytearray()
+
+    def slice(self, b: bytes) -> int:
+        off = len(self.pool)
+        self.pool += b
+        return off << 32 | len(b)
+
+
+def _pool(out) -> _Program:
+    if not isinstance(out, _Program):
+        raise TypeError("string tests are emitted through CompiledExpr")
+    return out
+
+
+_FLIP = {"EQ": "EQ", "LT": "GT", "LE": "GE", "GT": "LT", "GE": "LE"}
+
+
+def _utf8(v) -> bytes:
+    return v if isinstance(v, bytes) else v.encode("utf-8")
+
+
+def _is_str_lit(e) -> bool:
+    return isinstance(e, Literal) and isinstance(e.value, (str, bytes))
+
+
+def _string_col(c, schema) -> int:
+    i = schema.index(c.name)
+    if schema.types[i] != capi.SB_STRING:
+        raise TypeError("%r is not a string column" % c.name)
+    return i
+
+
+class _StringTest(Expression):
+    op = None
+    name = None
+
+    def __init__(self, child, literal):
+        if not isinstance(child, AttributeReference):
+            raise TypeError("string tests take a string column")
+        self.child, self.literal = child, _utf8(literal)
+        self.children = (child,)
+
+    def vtype(self, schema):
+        return VT_BOOL
+
+    def emit(self, schema, out):
+        out.append(_node(self.op, self.vtype(schema), _string_col(self.child, schema), lit_i=_pool(out).slice(self.literal)))
+
+    def sexpr(self):
+        return (self.name, self.child.sexpr(), self.literal)
+
+
+class StartsWith(_StringTest):
+    op, name = "STR_STARTS_WITH", "starts_with"
+
+
+class EndsWith(_StringTest):
+    op, name = "STR_ENDS_WITH", "ends_with"
+
+
+class Contains(_StringTest):
+    op, name = "STR_CONTAINS", "contains"
+
+
+class Like(_StringTest):
+    """`child LIKE pattern ESCAPE escape`: `_` one code point, `%` any run of them; the escape character may only precede `%`, `_`
+    or itself (the engine refuses other patterns with SB_ERR_INVALID)."""
+    op, name = "STR_LIKE", "like"
+
+    def __init__(self, child, pattern, escape="\\"):
+        super().__init__(child, pattern)
+        if len(escape) != 1:
+            raise ValueError("the escape must be one character")
+        self.escape = escape
+
+    def emit(self, schema, out):
+        out.append(_node(self.op, VT_BOOL, _string_col(self.child, schema), lit_i=_pool(out).slice(self.literal), arg2=ord(self.escape)))
+
+    def sexpr(self):
+        return ("like", self.child.sexpr(), self.literal.decode("utf-8"), self.escape)
+
+
+class In(_StringTest):
+    """`child IN (values)` over string literals; a None among them makes a miss NULL instead of FALSE."""
+    op, name = "STR_IN", "in"
+
+    def __init__(self, child, values):
+        super().__init__(child, b"")
+        self.values = [None if v is None else _utf8(v) for v in values]
+
+    def emit(self, schema, out):
+        lits = [v for v in self.values if v is not None]
+        blob = struct.pack("=I", len(lits)) + b"".join(struct.pack("=I", len(v)) + v for v in lits)
+        out.append(_node(self.op, VT_BOOL, _string_col(self.child, schema), lit_i=_pool(out).slice(blob),
+                         arg2=1 if None in self.values else 0))
+
+    def sexpr(self):
+        return ("in", self.child.sexpr(), list(self.values))
+
+
+class OctetLength(_StringTest):
+    op, name = "STR_OCTET_LENGTH", "octet_length"
+
+    def __init__(self, child):
+        super().__init__(child, b"")
+
+    def vtype(self, schema):
+        return VT_I32
+
+    def emit(self, schema, out):
+        out.append(_node(self.op, VT_I32, _string_col(self.child, schema)))
+
+    def sexpr(self):
+        return ("octet_length", self.child.sexpr())
+
+
 class CompiledExpr:
-    """Owns the ctypes arrays behind one sb_expr."""
+    """Owns the ctypes arrays behind one sb_expr: the nodes and the pool of string literals."""
 
     def __init__(self, expr: Expression, schema: Schema):
-        nodes = []
+        nodes = _Program()
         expr.emit(schema, nodes)
         self.arr = (capi.sb_expr_node * len(nodes))(*nodes)
         self.c = capi.sb_expr()
         self.c.nodes = C.cast(self.arr, C.POINTER(capi.sb_expr_node))
         self.c.n = len(nodes)
+        self.pool = (C.c_uint8 * max(1, len(nodes.pool))).from_buffer_copy(bytes(nodes.pool) or b"\0")
+        self.c.bytes = C.cast(self.pool, C.c_void_p) if nodes.pool else None
+        self.c.nbytes = len(nodes.pool)
         if isinstance(expr, AttributeReference):
             self.c.out_type = schema.types[schema.index(expr.name)]
         else:
