@@ -175,11 +175,15 @@ int sb_dictionary_decode(const sb_table *codes, int32_t col, const sb_table *dic
 #define SB_ENC_PLAIN 0
 #define SB_ENC_RLE_DICTIONARY 1   /* Parquet RLE_DICTIONARY / PLAIN_DICTIONARY data page: [bit width][RLE / bit-packed hybrid runs] */
 #define SB_ENC_RLE_BOOLEAN 2      /* BOOLEAN values as [4-byte length][hybrid runs, bit width 1] (data page V2 writers) */
+#define SB_ENC_DELTA_BINARY_PACKED 3      /* INT32 / INT64: [header][blocks of zig-zag min delta, bit widths, packed miniblocks] */
+#define SB_ENC_DELTA_LENGTH_BYTE_ARRAY 4  /* BYTE_ARRAY: DELTA_BINARY_PACKED lengths, then the concatenated bytes */
+#define SB_ENC_DELTA_BYTE_ARRAY 5         /* BYTE_ARRAY: DELTA_BINARY_PACKED prefix lengths, then DELTA_LENGTH_BYTE_ARRAY suffixes */
 #define SB_PHYS_BOOLEAN 0         /* Parquet physical types (parquet.thrift Type) */
 #define SB_PHYS_INT32 1
 #define SB_PHYS_INT64 2
 #define SB_PHYS_FLOAT 4
 #define SB_PHYS_DOUBLE 5
+#define SB_PHYS_BYTE_ARRAY 6      /* decodes to SB_STRING: PLAIN, dictionary, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY */
 
 typedef struct sb_page {            /* one data page; offsets are relative to sb_column_chunk.data */
   int32_t encoding;                 /* SB_ENC_* */
@@ -202,10 +206,15 @@ typedef struct sb_column_chunk {
 } sb_column_chunk;
 
 /* host only (no device): page descriptors of a column chunk lying in a Parquet file: Thrift compact PageHeader walk (data page
- * V1 / V2, dictionary page); compressed pages -> SB_ERR_UNSUPPORTED */
+ * V1 / V2, dictionary page); compressed pages -> SB_ERR_UNSUPPORTED.  The DELTA_BINARY_PACKED header in front of a DELTA_* page's
+ * values is validated here (block size in [1, 2^20], miniblock count in [1, block size], miniblock size a multiple of 8, total
+ * count not above the page's values: else SB_ERR_INVALID); a DELTA_BYTE_ARRAY page whose first prefix length is not 0 (it would
+ * continue the previous page's last value, PARQUET-246) -> SB_ERR_UNSUPPORTED. */
 int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int32_t max_def_level, sb_page *out_pages, int32_t pages_cap,
                            int32_t *out_npages, int64_t *out_dict_offset, int32_t *out_dict_count);
-/* one H2D copy per column chunk, then one decode kernel (a block per page) */
+/* one H2D copy per column chunk, then one decode kernel (a block per page).  A call with only fixed-width columns does not
+ * synchronise the stream.  A call that decodes SB_STRING columns (physical BYTE_ARRAY) synchronises it once, to read back the
+ * arena sizes of all of them together; an arena above 2^31 - 1 bytes is SB_ERR_UNSUPPORTED. */
 int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out);
 /* write-side twin (tests, bench.py): one NULL-free fixed-width column -> a column chunk on the device (out_chunk: one SB_INT8
  * column of bytes) + page descriptors on the host.  dictionary: one-column table of the distinct values in ascending order,

@@ -46,8 +46,9 @@ class sb_column_chunk(C.Structure):
                 ("data_bytes", C.c_int64), ("pages", C.POINTER(sb_page)), ("dict_offset", C.c_int64), ("dict_count", C.c_int32), ("pad", C.c_int32)]
 
 
-SB_ENC_PLAIN, SB_ENC_RLE_DICTIONARY = 0, 1
-SB_PHYS = dict(BOOLEAN=0, INT32=1, INT64=2, FLOAT=4, DOUBLE=5)
+SB_ENC_PLAIN, SB_ENC_RLE_DICTIONARY, SB_ENC_RLE_BOOLEAN = 0, 1, 2
+SB_ENC_DELTA_BINARY_PACKED, SB_ENC_DELTA_LENGTH_BYTE_ARRAY, SB_ENC_DELTA_BYTE_ARRAY = 3, 4, 5
+SB_PHYS = dict(BOOLEAN=0, INT32=1, INT64=2, FLOAT=4, DOUBLE=5, BYTE_ARRAY=6)
 
 
 class _lit(C.Union):

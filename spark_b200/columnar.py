@@ -267,7 +267,9 @@ class ColumnarBatch:
             if d.type == capi.SB_STRING:
                 offs, data = vals
                 vb = None if valid is None else pa.py_buffer(np.packbits(valid, bitorder="little").tobytes())
-                arr = pa.Array.from_buffers(pa.string(), int(d.length), [vb, pa.py_buffer(offs.tobytes()), pa.py_buffer(data.tobytes())])
+                at = self.arrow_types[i] if i < len(self.arrow_types) else None
+                typ = pa.binary() if at is not None and (pa.types.is_binary(at) or pa.types.is_large_binary(at)) else pa.string()
+                arr = pa.Array.from_buffers(typ, int(d.length), [vb, pa.py_buffer(offs.tobytes()), pa.py_buffer(data.tobytes())])
             elif d.type in (capi.SB_DECIMAL64, capi.SB_DECIMAL128):
                 n = int(d.length)
                 prec, scale = (d.scale >> 8) & 0xff, d.scale & 0xff

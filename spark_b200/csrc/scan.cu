@@ -10,11 +10,12 @@
 // Here the ENCODED page bytes cross PCIe (one copy per column chunk) and the GPU decodes them: for TPC-H lineitem the
 // dictionary-encoded columns are 1-12 bits per value instead of 8-64, which is what the end-to-end rate is bound by.
 //
-// Supported: physical types BOOLEAN / INT32 / INT64 / FLOAT / DOUBLE; encodings PLAIN and RLE_DICTIONARY (= PLAIN_DICTIONARY:
-// bit-width byte + hybrid runs over a PLAIN dictionary page); data pages V1 (levels length-prefixed in front of the values)
-// and V2 (levels in their own section); flat schemas (max definition level <= 1, no repetition); uncompressed pages (the
-// codec is the file writer's choice; decompression is not part of this path).  BYTE_ARRAY and DELTA_* are rejected with
-// SB_ERR_UNSUPPORTED rather than decoded on the CPU.
+// Supported: physical types BOOLEAN / INT32 / INT64 / FLOAT / DOUBLE, and BYTE_ARRAY decoded to SB_STRING; encodings PLAIN,
+// RLE_DICTIONARY (= PLAIN_DICTIONARY: bit-width byte + hybrid runs over a PLAIN dictionary page), DELTA_BINARY_PACKED (INT32 /
+// INT64), DELTA_LENGTH_BYTE_ARRAY and DELTA_BYTE_ARRAY (BYTE_ARRAY); data pages V1 (levels length-prefixed in front of the
+// values) and V2 (levels in their own section); flat schemas (max definition level <= 1, no repetition); uncompressed pages
+// (the codec is the file writer's choice; decompression is not part of this path).  FIXED_LEN_BYTE_ARRAY, INT96 and
+// BYTE_STREAM_SPLIT are rejected with SB_ERR_UNSUPPORTED rather than decoded on the CPU.
 //
 // Kernel: one 256-thread block per page.  (1) definition levels -> one validity byte per row; (2) values -> dense value
 // space (page-local), PLAIN by a widening/narrowing copy, RLE_DICTIONARY by walking the hybrid stream: thread 0 parses up
@@ -183,11 +184,297 @@ __device__ int64_t hybrid_decode(const uint8_t *__restrict__ p, int64_t nbytes, 
   return produced;
 }
 
+// definition levels of one page -> one validity byte per row (block-cooperative)
+__device__ void decode_validity(const PageTask &pg, uint8_t *vb, bool page_nullable) {
+  const int64_t n = pg.num_values;
+  if (page_nullable) {
+    const int64_t got = hybrid_decode(pg.def, pg.def_bytes, 1, n, 0, 1, [&](int64_t i, uint64_t v) { vb[i] = (uint8_t)(v & 1); });
+    for (int64_t i = got + threadIdx.x; i < n; i += SCAN_THREADS) vb[i] = 0;
+  } else {
+    for (int64_t i = threadIdx.x; i < n; i += SCAN_THREADS) vb[i] = 1;
+  }
+  __syncthreads();
+}
+
+// value space -> row space: put(row, valid, idx) for every row of the page, idx = number of valid rows before it (a block
+// scan of the validity bytes, PER rows per thread per tile)
+template <class Put>
+__device__ void expand_rows(const uint8_t *vb, int64_t n, Put put) {
+  __shared__ int s_warp[SCAN_THREADS / 32];
+  __shared__ int64_t s_base;
+  const int tid = threadIdx.x;
+  if (tid == 0) s_base = 0;
+  __syncthreads();
+  constexpr int PER = 4;
+  for (int64_t tile = 0; tile < n; tile += SCAN_THREADS * PER) {
+    const int64_t r0 = tile + (int64_t)tid * PER;
+    int cnt = 0;
+    uint8_t v[PER];
+#pragma unroll
+    for (int k = 0; k < PER; k++) {
+      v[k] = r0 + k < n ? vb[r0 + k] : 0;
+      cnt += v[k];
+    }
+    int incl = cnt;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      int o = __shfl_up_sync(0xffffffffu, incl, d);
+      if ((tid & 31) >= d) incl += o;
+    }
+    if ((tid & 31) == 31) s_warp[tid >> 5] = incl;
+    __syncthreads();
+    int wbase = 0;
+    for (int w = 0; w < (tid >> 5); w++) wbase += s_warp[w];
+    int total = 0;
+    for (int w = 0; w < SCAN_THREADS / 32; w++) total += s_warp[w];
+    int64_t idx = s_base + wbase + incl - cnt;
+#pragma unroll
+    for (int k = 0; k < PER; k++) {
+      if (r0 + k >= n) break;
+      put(r0 + k, v[k] != 0, idx);
+      if (v[k]) idx++;
+    }
+    __syncthreads();
+    if (tid == 0) s_base += total;
+    __syncthreads();
+  }
+}
+
+// fixed-width values: row r of the page takes dense[#valid rows before r], NULL rows 0
+__device__ void expand_fixed(const uint8_t *vb, int64_t n, const void *dense, void *dst_page, int ow) {
+  expand_rows(vb, n, [&](int64_t r, bool valid, int64_t idx) {
+    uint64_t val = 0;
+    if (valid) {
+      switch (ow) {
+        case 1: val = ((const uint8_t *)dense)[idx]; break;
+        case 2: val = ((const uint16_t *)dense)[idx]; break;
+        case 4: val = ((const uint32_t *)dense)[idx]; break;
+        default: val = ((const uint64_t *)dense)[idx]; break;
+      }
+    }
+    store_value(dst_page, ow, r, val);
+  });
+}
+
+// inclusive block scan of one 64-bit value per thread (wrapping); *total = sum over the block.  All threads call it.
+__device__ __forceinline__ uint64_t block_scan_u64(uint64_t x, uint64_t *total) {
+  __shared__ uint64_t s_w[SCAN_THREADS / 32];
+  const int tid = threadIdx.x, lane = tid & 31;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint64_t o = __shfl_up_sync(0xffffffffu, x, d);
+    if (lane >= d) x += o;
+  }
+  if (lane == 31) s_w[tid >> 5] = x;
+  __syncthreads();
+  uint64_t base = 0, tot = 0;
+  for (int w = 0; w < SCAN_THREADS / 32; w++) {
+    if (w < (tid >> 5)) base += s_w[w];
+    tot += s_w[w];
+  }
+  __syncthreads();
+  *total = tot;
+  return base + x;
+}
+
+// unsigned LEB128 of up to 64 bits (bounded by nbytes)
+__device__ __forceinline__ uint64_t read_uvarint64(const uint8_t *__restrict__ p, int64_t pos, int64_t nbytes, int *len) {
+  uint64_t v = 0;
+  int shift = 0, l = 0;
+  while (pos + l < nbytes) {
+    const uint8_t b = p[pos + l++];
+    if (shift < 64) v |= (uint64_t)(b & 0x7f) << shift;
+    shift += 7;
+    if (!(b & 0x80) || l >= 10) break;
+  }
+  *len = l;
+  return v;
+}
+__device__ __forceinline__ uint64_t unzigzag(uint64_t u) { return (u >> 1) ^ (0ull - (u & 1)); }
+
+// bw (<= 64) bits starting at bit `bit` of p[0..nbytes); bytes past the end read as 0
+__device__ __forceinline__ uint64_t unpack_bits(const uint8_t *__restrict__ p, int64_t nbytes, uint64_t bit, int bw) {
+  if (bw == 0) return 0;
+  const int64_t byte = (int64_t)(bit >> 3);
+  const int sh = (int)(bit & 7);
+  const int need = (sh + bw + 7) >> 3;   // <= 9
+  const int64_t left = nbytes - byte;
+  const int lo_n = (int)(left <= 0 ? 0 : (left < 8 ? left : 8));
+  uint64_t v = load_le(p + byte, lo_n < need ? lo_n : (need < 8 ? need : 8)) >> sh;
+  if (need > 8 && left > 8) v |= (uint64_t)p[byte + 8] << (64 - sh);
+  return bw >= 64 ? v : (v & ((1ull << bw) - 1));
+}
+
+// DELTA_BINARY_PACKED (VectorizedDeltaBinaryPackedReader.java): header <block size><miniblocks per block><total count><zig-zag first
+// value>, then blocks of <zig-zag min delta><one bit-width byte per miniblock><packed miniblocks>; value i+1 = value i + min delta +
+// packed delta, wrapping in 64 bits.  In the last block the bit-width bytes of unused miniblocks are present, their bodies are
+// not.  Block-cooperative, in the manner of hybrid_decode: warp 0's lane 0 walks the miniblock headers (one byte each, plus a
+// varint per block) into a batch of up to SCAN_RUNS miniblocks; the block decodes the batch's deltas (delta i finds its miniblock
+// by binary search) and turns them into values with a block scan carried across tiles.  emit(i, v) for i < max_values (values the
+// stream does not hold are emitted as 0); returns the byte position where the stream ends (the whole stream is walked, also when
+// max_values is smaller), the same in every thread.
+template <class Emit>
+__device__ int64_t dbp_decode(const uint8_t *__restrict__ p, int64_t nbytes, int64_t max_values, Emit emit) {
+  __shared__ int64_t s_off[SCAN_RUNS];      // byte offset of the miniblock's body
+  __shared__ uint64_t s_min[SCAN_RUNS];
+  __shared__ uint8_t s_bw[SCAN_RUNS];
+  __shared__ uint32_t s_pref[SCAN_RUNS + 1];
+  __shared__ int s_n;
+  __shared__ int64_t s_pos, s_walked, s_bwpos, s_done_total, s_decoded;
+  __shared__ uint64_t s_carry, s_bmin;
+  __shared__ int s_m, s_minis, s_vpm;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    int l;
+    int64_t pos = 0;
+    const uint64_t block = read_uvarint64(p, pos, nbytes, &l); pos += l;
+    const uint64_t minis = read_uvarint64(p, pos, nbytes, &l); pos += l;
+    const uint64_t total = read_uvarint64(p, pos, nbytes, &l); pos += l;
+    const uint64_t first = unzigzag(read_uvarint64(p, pos, nbytes, &l)); pos += l;
+    // the page walker validated the header of every page it described; a hand-built descriptor gets the same limits here
+    const bool ok = block >= 1 && block <= (1u << 20) && minis >= 1 && minis <= block && (block / minis) % 8 == 0 && block % minis == 0;
+    s_minis = ok ? (int)minis : 1;
+    s_vpm = ok ? (int)(block / minis) : 0;
+    s_m = s_minis;                                   // no block open yet
+    s_done_total = ok && total > 0 ? (int64_t)(total < (1ull << 40) ? total : (1ull << 40)) - 1 : 0;   // deltas in the stream
+    s_walked = 0;
+    s_pos = pos;
+    s_carry = first;
+    s_decoded = ok && total > 0 && max_values > 0 ? 1 : 0;
+    if (s_decoded) emit(0, first);
+  }
+  __syncthreads();
+  const int64_t want = max_values - 1;             // deltas to decode
+  while (true) {
+    if (tid == 0) {
+      int n = 0;
+      uint32_t acc = 0;
+      int64_t pos = s_pos, walked = s_walked, bwpos = s_bwpos;
+      int m = s_m;
+      const int minis = s_minis, vpm = s_vpm;
+      const int64_t total = s_done_total;
+      uint64_t bmin = s_bmin;
+      s_pref[0] = 0;
+      while (walked < total && n < SCAN_RUNS && acc < (1u << 30)) {
+        if (m == minis) {                            // next block: min delta, then the bit widths of all its miniblocks
+          if (pos >= nbytes) { walked = total; break; }
+          int l;
+          bmin = unzigzag(read_uvarint64(p, pos, nbytes, &l));
+          bwpos = pos + l;
+          pos = bwpos + minis;
+          m = 0;
+        }
+        int bw = bwpos + m < nbytes ? p[bwpos + m] : 0;
+        if (bw > 64) bw = 64;
+        const int64_t cnt = total - walked < vpm ? total - walked : vpm;
+        if (walked < want) {
+          const int64_t take = want - walked < cnt ? want - walked : cnt;
+          s_off[n] = pos;
+          s_min[n] = bmin;
+          s_bw[n] = (uint8_t)bw;
+          acc += (uint32_t)take;
+          s_pref[n + 1] = acc;
+          n++;
+        }
+        pos += (int64_t)vpm * bw / 8;                // a miniblock that holds any value is stored whole
+        walked += cnt;
+        m++;
+      }
+      s_n = n;
+      s_pos = pos < nbytes ? pos : nbytes;
+      s_walked = walked;
+      s_bwpos = bwpos;
+      s_m = m;
+      s_bmin = bmin;
+    }
+    __syncthreads();
+    const int nm = s_n;
+    if (nm == 0) break;
+    const uint32_t bt = s_pref[nm];
+    const int64_t base = s_decoded;
+    for (uint32_t t0 = 0; t0 < bt; t0 += SCAN_THREADS) {
+      const uint32_t i = t0 + tid;
+      uint64_t d = 0;
+      if (i < bt) {
+        int lo = 0, hi = nm;                         // last miniblock with pref <= i
+        while (hi - lo > 1) {
+          const int mid = (lo + hi) >> 1;
+          if (s_pref[mid] <= i) lo = mid; else hi = mid;
+        }
+        const int bw = s_bw[lo];
+        d = s_min[lo] + unpack_bits(p + s_off[lo], nbytes - s_off[lo], (uint64_t)(i - s_pref[lo]) * (uint64_t)bw, bw);
+      }
+      uint64_t tot;
+      const uint64_t v = s_carry + block_scan_u64(d, &tot);
+      if (i < bt) emit(base + i, v);
+      __syncthreads();
+      if (tid == 0) s_carry += tot;
+      __syncthreads();
+    }
+    if (tid == 0) s_decoded += bt;
+    __syncthreads();
+  }
+  for (int64_t i = s_decoded + tid; i < max_values; i += SCAN_THREADS) emit(i, 0ull);
+  const int64_t end = s_pos;
+  __syncthreads();
+  return end;
+}
+
+// PLAIN byte arrays (VectorizedPlainValuesReader.readBinary): [4-byte LE length][bytes] per value.  The lengths form a chain, so
+// one thread walks it, but over a window of the page staged in shared memory by the whole block: one HBM round trip per window,
+// not per value.  A value larger than the window moves the next window to the length that follows it.  Lengths are clamped
+// to the bytes left.  emit(k, offset of the bytes, length) for the first max_values values; returns how many there were.
+constexpr int PLAIN_WINDOW = 8192;
+template <class Emit>
+__device__ int64_t plain_walk(const uint8_t *__restrict__ p, int64_t nbytes, int64_t max_values, Emit emit) {
+  __shared__ uint8_t s_win[PLAIN_WINDOW];
+  __shared__ int64_t s_pos, s_k;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    s_pos = 0;
+    s_k = 0;
+  }
+  __syncthreads();
+  while (true) {
+    const int64_t w0 = s_pos, k0 = s_k;
+    if (k0 >= max_values || w0 + 4 > nbytes) break;
+    const int64_t wn = nbytes - w0 < PLAIN_WINDOW ? nbytes - w0 : PLAIN_WINDOW;
+    for (int64_t i = tid; i < wn; i += SCAN_THREADS) s_win[i] = p[w0 + i];
+    __syncthreads();
+    if (tid == 0) {
+      int64_t pos = w0, k = k0;
+      while (k < max_values && pos + 4 <= nbytes && pos + 4 <= w0 + wn) {
+        const uint8_t *h = s_win + (pos - w0);
+        const int64_t len = (int64_t)((uint32_t)h[0] | ((uint32_t)h[1] << 8) | ((uint32_t)h[2] << 16) | ((uint32_t)h[3] << 24));
+        const int64_t left = nbytes - pos - 4;
+        const int64_t l = len < left ? len : left;
+        emit(k, pos + 4, (int32_t)l);
+        pos += 4 + l;
+        k++;
+      }
+      s_pos = pos;
+      s_k = k;
+    }
+    __syncthreads();
+  }
+  const int64_t got = s_k;
+  __syncthreads();
+  return got;
+}
+
+// number of non-zero validity bytes of a page
+__device__ int64_t count_valid(const uint8_t *vb, int64_t n) {
+  int64_t c = 0;
+  for (int64_t i = threadIdx.x; i < n; i += SCAN_THREADS) c += vb[i];
+  uint64_t tot;
+  block_scan_u64((uint64_t)c, &tot);
+  return (int64_t)tot;
+}
+
 __global__ void __launch_bounds__(SCAN_THREADS) scan_decode_kernel(const PageTask *__restrict__ pages, const ColTask *__restrict__ cols, int nparts) {
   const PageTask pg = pages[blockIdx.x / nparts];
   int part = blockIdx.x % nparts;
   const ColTask c = cols[pg.col];
-  const int tid = threadIdx.x;
   const int64_t n = pg.num_values;
   // ---- (1) definition levels -> validity bytes -------------------------------------------------------------------------
   uint8_t *vb = c.valid_bytes ? c.valid_bytes + pg.row_start : nullptr;
@@ -196,15 +483,8 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_decode_kernel(const PageTas
     if (part != 0) return;
     nparts = 1;
   }
-  if (vb && part == 0) {
-    if (page_nullable) {
-      const int64_t got = hybrid_decode(pg.def, pg.def_bytes, 1, n, 0, 1, [&](int64_t i, uint64_t v) { vb[i] = (uint8_t)(v & 1); });
-      for (int64_t i = got + tid; i < n; i += SCAN_THREADS) vb[i] = 0;
-    } else {
-      for (int64_t i = tid; i < n; i += SCAN_THREADS) vb[i] = 1;
-    }
-    __syncthreads();
-  }
+  if (vb && part == 0) decode_validity(pg, vb, page_nullable);
+  const int tid = threadIdx.x;
   // ---- (2) values -> dense value space (or straight to the output when the page has no NULLs) -----------------------------
   void *dst_page = (uint8_t *)c.out + pg.row_start * c.out_width;
   void *dense = page_nullable ? (void *)(c.dense + pg.row_start * c.out_width) : dst_page;
@@ -247,51 +527,217 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_decode_kernel(const PageTas
   if (!page_nullable) return;
   __syncthreads();
   // ---- (3) expand value space -> row space: row r takes dense[#valid rows before r] --------------------------------------
-  __shared__ int s_warp[SCAN_THREADS / 32];
-  __shared__ int64_t s_base;
-  if (tid == 0) s_base = 0;
+  expand_fixed(vb, n, dense, dst_page, ow);
+}
+
+// DELTA_BINARY_PACKED pages of INT32 / INT64 columns, one block per page, steps (1)-(3) of scan_decode_kernel around dbp_decode
+// (a kernel of its own so that the hybrid decoder's kernel keeps its registers)
+__global__ void __launch_bounds__(SCAN_THREADS) scan_delta_kernel(const PageTask *__restrict__ pages, const ColTask *__restrict__ cols) {
+  const PageTask pg = pages[blockIdx.x];
+  const ColTask c = cols[pg.col];
+  const int64_t n = pg.num_values;
+  uint8_t *vb = c.valid_bytes ? c.valid_bytes + pg.row_start : nullptr;
+  const bool page_nullable = pg.def != nullptr && pg.def_bytes > 0;
+  if (vb) decode_validity(pg, vb, page_nullable);
+  const int ow = c.out_width, pw = c.phys_width;
+  void *dst_page = (uint8_t *)c.out + pg.row_start * ow;
+  void *dense = page_nullable ? (void *)(c.dense + pg.row_start * ow) : dst_page;
+  dbp_decode(pg.values, pg.values_bytes, n, [&](int64_t i, uint64_t v) {   // 64-bit running sum, truncated to the column's width
+    if (pw == 4 && ow == 8) v = (uint64_t)(int64_t)(int32_t)v;
+    store_value(dense, ow, i, v);
+  });
+  if (!page_nullable) return;
   __syncthreads();
-  constexpr int PER = 4;
-  for (int64_t tile = 0; tile < n; tile += SCAN_THREADS * PER) {
-    const int64_t r0 = tile + (int64_t)tid * PER;
-    int cnt = 0;
-    uint8_t v[PER];
-#pragma unroll
-    for (int k = 0; k < PER; k++) {
-      v[k] = r0 + k < n ? vb[r0 + k] : 0;
-      cnt += v[k];
+  expand_fixed(vb, n, dense, dst_page, ow);
+}
+
+// ---- BYTE_ARRAY -> SB_STRING --------------------------------------------------------------------------------------------
+// (a) str_dict_kernel: one block per dictionary chunk walks its PLAIN dictionary page into (offset, length) entries.
+// (b) str_page_kernel: one block per page: validity, then every value's (length, source offset in the chunk, prefix length) in
+//     value space, expanded to row space (NULL rows: length 0).
+// (c) host: exclusive scan of the lengths -> int64 offsets; ONE stream synchronisation reads back the arena sizes of all string
+//     columns of the call (Column::string_bytes is exact on the host); an arena above 2^31 - 1 bytes is refused.
+// (d) str_copy_kernel: row-parallel, one warp per 32 rows: the bytes each value takes from its page (DELTA_BYTE_ARRAY: the
+//     suffix, after the prefix) and the int32 offsets.
+// (e) str_prefix_kernel: one warp per DELTA_BYTE_ARRAY page, in value order: value i's first prefix[i] bytes from value i-1.
+struct StrColTask {
+  const uint8_t *base;                 // device chunk
+  uint8_t *valid_bytes;                // or nullptr
+  int32_t *vlen, *vpre;                // value space (NULLable columns) or the row arrays themselves
+  int64_t *vsrc;
+  int32_t *rlen, *rpre;                // row space; rpre nullptr unless a page is DELTA_BYTE_ARRAY
+  int64_t *rsrc;
+  int32_t *dict_len;                   // dictionary entries
+  int64_t *dict_src;
+  int64_t dict_offset, data_bytes;
+  int32_t dict_count;
+  int32_t pad;
+};
+struct StrOutTask {
+  const int64_t *off;                  // exclusive scan of rlen
+  int32_t *out_off;                    // column offsets (rows + 1)
+  uint8_t *arena;
+  int64_t nrows;
+};
+
+__global__ void __launch_bounds__(SCAN_THREADS) str_dict_kernel(const StrColTask *__restrict__ cols, const int32_t *__restrict__ which) {
+  const StrColTask c = cols[which[blockIdx.x]];
+  const int64_t got = plain_walk(c.base + c.dict_offset, c.data_bytes - c.dict_offset, c.dict_count, [&](int64_t k, int64_t off, int32_t len) {
+    c.dict_len[k] = len;
+    c.dict_src[k] = c.dict_offset + off;
+  });
+  for (int64_t k = got + threadIdx.x; k < c.dict_count; k += SCAN_THREADS) {
+    c.dict_len[k] = 0;
+    c.dict_src[k] = 0;
+  }
+}
+
+// DELTA_LENGTH_BYTE_ARRAY section at p[0..nbytes): lengths, then the bytes; lens[i] clamped so that value i lies inside the section.
+// Writes lens / src (chunk offsets: p is at chunk offset p_off) for i < nvals; returns the section's end.
+__device__ int64_t dlba_decode(const uint8_t *p, int64_t nbytes, int64_t p_off, int64_t nvals, int32_t *lens, int64_t *src) {
+  const int64_t start = dbp_decode(p, nbytes, nvals, [&](int64_t i, uint64_t v) {
+    lens[i] = (int64_t)v < 0 ? 0 : ((int64_t)v > 0x7fffffff ? 0x7fffffff : (int32_t)v);
+  });
+  __syncthreads();
+  __shared__ int64_t s_run;
+  if (threadIdx.x == 0) s_run = start;
+  __syncthreads();
+  for (int64_t t0 = 0; t0 < nvals; t0 += SCAN_THREADS) {
+    const int64_t i = t0 + threadIdx.x;
+    const int64_t l = i < nvals ? lens[i] : 0;
+    uint64_t tot;
+    const int64_t at = s_run + (int64_t)block_scan_u64((uint64_t)l, &tot) - l;
+    if (i < nvals) {
+      const int64_t s = at < nbytes ? at : nbytes;
+      lens[i] = (int32_t)(s + l <= nbytes ? l : nbytes - s);
+      src[i] = p_off + s;
     }
-    int incl = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      int o = __shfl_up_sync(0xffffffffu, incl, d);
-      if ((tid & 31) >= d) incl += o;
-    }
-    if ((tid & 31) == 31) s_warp[tid >> 5] = incl;
     __syncthreads();
-    int wbase = 0;
-    for (int w = 0; w < (tid >> 5); w++) wbase += s_warp[w];
-    int total = 0;
-    for (int w = 0; w < SCAN_THREADS / 32; w++) total += s_warp[w];
-    int64_t idx = s_base + wbase + incl - cnt;
+    if (threadIdx.x == 0) s_run += (int64_t)tot;
+    __syncthreads();
+  }
+  const int64_t end = s_run < nbytes ? s_run : nbytes;
+  __syncthreads();
+  return end;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) str_page_kernel(const PageTask *__restrict__ pages, const StrColTask *__restrict__ cols) {
+  const PageTask pg = pages[blockIdx.x];
+  const StrColTask c = cols[pg.col];
+  const int64_t n = pg.num_values;
+  uint8_t *vb = c.valid_bytes ? c.valid_bytes + pg.row_start : nullptr;
+  const bool page_nullable = pg.def != nullptr && pg.def_bytes > 0;
+  if (vb) decode_validity(pg, vb, page_nullable);
+  const int64_t nvals = page_nullable ? count_valid(vb, n) : n;
+  int32_t *vlen = (page_nullable ? c.vlen : c.rlen) + pg.row_start;
+  int64_t *vsrc = (page_nullable ? c.vsrc : c.rsrc) + pg.row_start;
+  int32_t *vpre = c.rpre ? (page_nullable ? c.vpre : c.rpre) + pg.row_start : nullptr;
+  const int64_t voff = pg.values - c.base;   // chunk offset of the page's values
+  int64_t got = nvals;
+  if (pg.encoding == SB_ENC_PLAIN) {
+    got = plain_walk(pg.values, pg.values_bytes, nvals, [&](int64_t k, int64_t off, int32_t len) {
+      vlen[k] = len;
+      vsrc[k] = voff + off;
+    });
+  } else if (pg.encoding == SB_ENC_RLE_DICTIONARY) {
+    const int bw = pg.values_bytes > 0 ? pg.values[0] : 0;
+    got = nvals > 0 ? hybrid_decode(pg.values + 1, pg.values_bytes - 1, bw > 32 ? 32 : bw, nvals, 0, 1, [&](int64_t i, uint64_t idx) {
+      const bool in = idx < (uint64_t)c.dict_count;
+      vlen[i] = in ? c.dict_len[idx] : 0;
+      vsrc[i] = in ? c.dict_src[idx] : 0;
+    }) : 0;
+  } else if (pg.encoding == SB_ENC_DELTA_LENGTH_BYTE_ARRAY) {
+    dlba_decode(pg.values, pg.values_bytes, voff, nvals, vlen, vsrc);
+  } else {   // DELTA_BYTE_ARRAY: prefix lengths, then DELTA_LENGTH_BYTE_ARRAY suffixes; the length is prefix + suffix
+    const int64_t pend = dbp_decode(pg.values, pg.values_bytes, nvals, [&](int64_t i, uint64_t v) {
+      vpre[i] = (int64_t)v < 0 ? 0 : ((int64_t)v > 0x7fffffff ? 0x7fffffff : (int32_t)v);
+    });
+    dlba_decode(pg.values + pend, pg.values_bytes - pend, voff + pend, nvals, vlen, vsrc);
+    for (int64_t i = threadIdx.x; i < nvals; i += SCAN_THREADS) {
+      const int64_t l = (int64_t)vlen[i] + vpre[i];
+      vlen[i] = (int32_t)(l > 0x7fffffff ? 0x7fffffff : l);
+    }
+  }
+  for (int64_t i = got + threadIdx.x; i < nvals; i += SCAN_THREADS) {   // values the page does not hold are empty
+    vlen[i] = 0;
+    vsrc[i] = 0;
+  }
+  if (vpre && pg.encoding != SB_ENC_DELTA_BYTE_ARRAY)
+    for (int64_t i = threadIdx.x; i < nvals; i += SCAN_THREADS) vpre[i] = 0;
+  if (!page_nullable) return;
+  __syncthreads();
+  int32_t *rlen = c.rlen + pg.row_start, *rpre = c.rpre ? c.rpre + pg.row_start : nullptr;
+  int64_t *rsrc = c.rsrc + pg.row_start;
+  expand_rows(vb, n, [&](int64_t r, bool valid, int64_t idx) {
+    rlen[r] = valid ? vlen[idx] : 0;
+    rsrc[r] = valid ? vsrc[idx] : 0;
+    if (rpre) rpre[r] = valid ? vpre[idx] : 0;
+  });
+}
+
+// bytes that come from the page: value r's [pre, len) from its source; 8 loads in flight per lane
+__global__ void __launch_bounds__(SCAN_THREADS) str_copy_kernel(StrColTask c, StrOutTask o) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * SCAN_THREADS + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * SCAN_THREADS) >> 5;
+  for (int64_t r0 = warp * 32; r0 < o.nrows; r0 += nwarps * 32) {
+    const int64_t r = r0 + lane;
+    int64_t off = 0, src = 0;
+    int32_t len = 0, pre = 0;
+    if (r < o.nrows) {
+      off = o.off[r];
+      len = c.rlen[r];
+      src = c.rsrc[r];
+      pre = c.rpre ? c.rpre[r] : 0;
+      if (pre > len) pre = len;
+      o.out_off[r] = (int32_t)off;
+    }
+    const int rows = o.nrows - r0 < 32 ? (int)(o.nrows - r0) : 32;
+    for (int k = 0; k < rows; k++) {
+      const int64_t koff = __shfl_sync(0xffffffffu, off, k) + __shfl_sync(0xffffffffu, pre, k);
+      const int64_t ksrc = __shfl_sync(0xffffffffu, src, k);
+      const int64_t klen = __shfl_sync(0xffffffffu, len, k) - __shfl_sync(0xffffffffu, pre, k);
+      const uint8_t *s = c.base + ksrc;
+      uint8_t *d = o.arena + koff;
+      for (int64_t b = lane; b < klen; b += 32 * 8) {
+        uint8_t v[8];
 #pragma unroll
-    for (int k = 0; k < PER; k++) {
-      if (r0 + k >= n) break;
-      uint64_t val = 0;
-      if (v[k]) {
-        switch (ow) {
-          case 1: val = ((const uint8_t *)dense)[idx]; break;
-          case 2: val = ((const uint16_t *)dense)[idx]; break;
-          case 4: val = ((const uint32_t *)dense)[idx]; break;
-          default: val = ((const uint64_t *)dense)[idx]; break;
-        }
-        idx++;
+        for (int u = 0; u < 8; u++) v[u] = b + 32 * u < klen ? s[b + 32 * u] : 0;
+#pragma unroll
+        for (int u = 0; u < 8; u++)
+          if (b + 32 * u < klen) d[b + 32 * u] = v[u];
       }
-      store_value(dst_page, ow, r0 + k, val);
     }
-    __syncthreads();
-    if (tid == 0) s_base += total;
-    __syncthreads();
+  }
+}
+
+// DELTA_BYTE_ARRAY prefixes, one warp per page in value order (VectorizedDeltaByteArrayReader.readValues): value i's first
+// prefix[i] bytes are value i-1's.  A prefix longer than the previous value (a malformed page) is filled with zero bytes.
+__global__ void str_prefix_kernel(const PageTask *__restrict__ pages, const StrColTask *__restrict__ cols, const StrOutTask *__restrict__ outs) {
+  const PageTask pg = pages[blockIdx.x];
+  const StrColTask c = cols[pg.col];
+  const StrOutTask o = outs[pg.col];
+  const int lane = threadIdx.x & 31;
+  int64_t prev_off = 0, prev_len = 0;
+  bool have_prev = false;
+  for (int64_t r0 = pg.row_start; r0 < pg.row_start + pg.num_values; r0 += 32) {
+    const int64_t r = r0 + lane;
+    const bool in = r < pg.row_start + pg.num_values;
+    const bool valid = in && (!c.valid_bytes || c.valid_bytes[r]);
+    const int64_t off = in ? o.off[r] : 0;
+    const int32_t len = in ? c.rlen[r] : 0, pre = in ? c.rpre[r] : 0;
+    const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+    for (int k = 0; k < 32; k++) {
+      if (!((vmask >> k) & 1)) continue;
+      const int64_t koff = __shfl_sync(0xffffffffu, off, k);
+      const int32_t klen = __shfl_sync(0xffffffffu, len, k);
+      int32_t kpre = __shfl_sync(0xffffffffu, pre, k);
+      if (kpre > klen) kpre = klen;
+      for (int32_t b = lane; b < kpre; b += 32) o.arena[koff + b] = have_prev && b < prev_len ? o.arena[prev_off + b] : 0;
+      __syncwarp();
+      prev_off = koff;
+      prev_len = klen;
+      have_prev = true;
+    }
   }
 }
 
@@ -458,6 +904,32 @@ bool read_page_header(Thrift &t, PageHeader &h) {
   }
   return false;
 }
+
+// The DELTA_BINARY_PACKED header in front of a DELTA_* page's values, validated as VectorizedDeltaBinaryPackedReader.initFromPage
+// does (:91-122); for DELTA_BYTE_ARRAY it is the prefix-length stream's.  That stream's first value is the first prefix length:
+// a page that does not start it at 0 continues the previous page's last value (PARQUET-246, VectorizedDeltaByteArrayReader
+// :76-80), which the per-page decode does not carry over, so the page is refused instead.
+void check_delta_header(const uint8_t *p, int64_t nbytes, int32_t enc, int64_t page_values, int page, int64_t page_pos) {
+  Thrift t{p, p + nbytes};
+  const uint64_t block = t.varint(), minis = t.varint(), total = t.varint();
+  const int64_t first = t.zigzag();
+  if (!t.ok) fail(SB_ERR_INVALID, "page %d (byte %lld of the column chunk): truncated DELTA_BINARY_PACKED header", page, (long long)page_pos);
+  if (block < 1 || block > (1u << 20))
+    fail(SB_ERR_INVALID, "page %d (byte %lld of the column chunk): DELTA_BINARY_PACKED block size %llu is not in [1, 2^20]", page, (long long)page_pos,
+         (unsigned long long)block);
+  if (minis < 1 || minis > block)
+    fail(SB_ERR_INVALID, "page %d (byte %lld of the column chunk): DELTA_BINARY_PACKED miniblock count %llu is not in [1, %llu]", page,
+         (long long)page_pos, (unsigned long long)minis, (unsigned long long)block);
+  if (block % minis != 0 || (block / minis) % 8 != 0)
+    fail(SB_ERR_INVALID, "page %d (byte %lld of the column chunk): DELTA_BINARY_PACKED miniblock size %llu / %llu is not a multiple of 8", page,
+         (long long)page_pos, (unsigned long long)block, (unsigned long long)minis);
+  if (total > (uint64_t)page_values)
+    fail(SB_ERR_INVALID, "page %d (byte %lld of the column chunk): DELTA_BINARY_PACKED total count %llu exceeds the page's %lld values", page,
+         (long long)page_pos, (unsigned long long)total, (long long)page_values);
+  if (enc == SB_ENC_DELTA_BYTE_ARRAY && total > 0 && first != 0)
+    fail(SB_ERR_UNSUPPORTED, "page %d (byte %lld of the column chunk): DELTA_BYTE_ARRAY page starts with prefix length %lld; continuing the "
+         "previous page's value (PARQUET-246) is not supported", page, (long long)page_pos, (long long)first);
+}
 }  // namespace
 
 // Host only (no device needed): walks the pages of one column chunk as it lies in a Parquet file (the byte range
@@ -492,7 +964,10 @@ extern "C" int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int3
       if (h.encoding == 0) pg.encoding = SB_ENC_PLAIN;
       else if (h.encoding == 2 || h.encoding == 8) pg.encoding = SB_ENC_RLE_DICTIONARY;
       else if (h.encoding == 3) pg.encoding = SB_ENC_RLE_BOOLEAN;   // only BOOLEAN columns may use it (checked in sb_scan_decode)
-      else fail(SB_ERR_UNSUPPORTED, "Parquet value encoding %d is not supported (PLAIN and RLE_DICTIONARY are)", h.encoding);
+      else if (h.encoding == 5) pg.encoding = SB_ENC_DELTA_BINARY_PACKED;
+      else if (h.encoding == 6) pg.encoding = SB_ENC_DELTA_LENGTH_BYTE_ARRAY;
+      else if (h.encoding == 7) pg.encoding = SB_ENC_DELTA_BYTE_ARRAY;
+      else fail(SB_ERR_UNSUPPORTED, "Parquet value encoding %d is not supported (PLAIN, RLE_DICTIONARY and the DELTA encodings are)", h.encoding);
       pg.num_values = h.num_values;
       int64_t vpos = body, vend = body + h.compressed;
       if (h.type == 0) {
@@ -515,6 +990,7 @@ extern "C" int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int3
       SB_REQUIRE(vpos <= vend, "Parquet page levels overrun the page");
       pg.values_offset = vpos;
       pg.values_bytes = vend - vpos;
+      if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED) check_delta_header(chunk + vpos, vend - vpos, pg.encoding, h.num_values, np - 1, pos);
     }   // INDEX_PAGE and unknown page types are skipped
     pos = body + h.compressed;
   }
@@ -531,6 +1007,80 @@ static int phys_width_of(int32_t physical) {
   fail(SB_ERR_UNSUPPORTED, "Parquet physical type %d is not supported by the GPU scan (BOOLEAN, INT32, INT64, FLOAT, DOUBLE are)", physical);
 }
 
+// host state of one sb_scan_decode call that the stream reads asynchronously (freed by a host function behind the kernels)
+struct ScanKeep {
+  std::vector<PageTask> tasks, delta_tasks, str_pages, dba_pages;
+  std::vector<ColTask> ctasks;
+  std::vector<StrColTask> stasks;
+  std::vector<StrOutTask> outs;
+  std::vector<int32_t> dict_cols, str_cols, totals32;
+  std::vector<int64_t> totals;
+};
+
+// steps (a)-(e) above for the string columns of one call; the one stream synchronisation of a call that decodes strings
+static void decode_strings(ScanKeep &k, sb_table *t, int64_t nrows, cudaStream_t st) {
+  const int ncols = (int)k.stasks.size(), nstr = (int)k.str_cols.size();
+  Scratch d_cols((int64_t)ncols * sizeof(StrColTask), st), d_pages((int64_t)k.str_pages.size() * sizeof(PageTask), st),
+      d_which((int64_t)k.dict_cols.size() * 4, st);
+  SB_CUDA(cudaMemcpyAsync(d_cols.ptr, k.stasks.data(), (size_t)ncols * sizeof(StrColTask), cudaMemcpyHostToDevice, st));
+  if (!k.str_pages.empty()) SB_CUDA(cudaMemcpyAsync(d_pages.ptr, k.str_pages.data(), k.str_pages.size() * sizeof(PageTask), cudaMemcpyHostToDevice, st));
+  if (!k.dict_cols.empty()) SB_CUDA(cudaMemcpyAsync(d_which.ptr, k.dict_cols.data(), k.dict_cols.size() * 4, cudaMemcpyHostToDevice, st));
+  {
+    KernelTimer kt("scan_decode_strings", st);
+    if (!k.dict_cols.empty()) {
+      str_dict_kernel<<<(unsigned)k.dict_cols.size(), SCAN_THREADS, 0, st>>>(d_cols.as<StrColTask>(), d_which.as<int32_t>());
+      SB_LAUNCH_CHECK();
+    }
+    if (!k.str_pages.empty()) {
+      str_page_kernel<<<(unsigned)k.str_pages.size(), SCAN_THREADS, 0, st>>>(d_pages.as<PageTask>(), d_cols.as<StrColTask>());
+      SB_LAUNCH_CHECK();
+    }
+  }
+  // (c) offsets and arena sizes
+  Scratch d_off((int64_t)nstr * (nrows + 1) * 8 + 16, st), d_tot((int64_t)nstr * 8 + 16, st);
+  k.totals.assign(nstr, 0);
+  if (nrows > 0) {
+    for (int j = 0; j < nstr; j++)
+      exclusive_scan_i32_to_i64(k.stasks[k.str_cols[j]].rlen, d_off.as<int64_t>() + (int64_t)j * (nrows + 1), nrows, d_tot.as<int64_t>() + j, st);
+    SB_CUDA(cudaMemcpyAsync(k.totals.data(), d_tot.ptr, (size_t)nstr * 8, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+  }
+  k.outs.assign(ncols, StrOutTask{});
+  k.totals32.assign(nstr, 0);
+  for (int j = 0; j < nstr; j++) {
+    const int ci = k.str_cols[j];
+    if (k.totals[j] > 0x7fffffffll)
+      fail(SB_ERR_UNSUPPORTED, "column chunk %d: the decoded strings take %lld bytes, more than the 2^31 - 1 an int32-offset string column holds", ci,
+           (long long)k.totals[j]);
+    Column &col = t->cols[ci];
+    col.data = buffer_alloc(k.totals[j] + 16, st);
+    col.string_bytes = k.totals[j];
+    k.totals32[j] = (int32_t)k.totals[j];
+    SB_CUDA(cudaMemcpyAsync((int32_t *)col.offsets->ptr + nrows, &k.totals32[j], 4, cudaMemcpyHostToDevice, st));
+    StrOutTask &o = k.outs[ci];
+    o.off = d_off.as<int64_t>() + (int64_t)j * (nrows + 1);
+    o.out_off = (int32_t *)col.offsets->ptr;
+    o.arena = (uint8_t *)col.data->ptr;
+    o.nrows = nrows;
+  }
+  if (nrows == 0) return;
+  // (d), (e) the bytes
+  KernelTimer kt("scan_copy_strings", st);
+  const int grid = grid_for(nrows, SCAN_THREADS, rt().num_sms * 16);
+  for (int j = 0; j < nstr; j++) {
+    const int ci = k.str_cols[j];
+    str_copy_kernel<<<grid, SCAN_THREADS, 0, st>>>(k.stasks[ci], k.outs[ci]);
+    SB_LAUNCH_CHECK();
+  }
+  if (!k.dba_pages.empty()) {
+    Scratch d_dba((int64_t)k.dba_pages.size() * sizeof(PageTask), st), d_outs((int64_t)ncols * sizeof(StrOutTask), st);
+    SB_CUDA(cudaMemcpyAsync(d_dba.ptr, k.dba_pages.data(), k.dba_pages.size() * sizeof(PageTask), cudaMemcpyHostToDevice, st));
+    SB_CUDA(cudaMemcpyAsync(d_outs.ptr, k.outs.data(), (size_t)ncols * sizeof(StrOutTask), cudaMemcpyHostToDevice, st));
+    str_prefix_kernel<<<(unsigned)k.dba_pages.size(), 32, 0, st>>>(d_dba.as<PageTask>(), d_cols.as<StrColTask>(), d_outs.as<StrOutTask>());
+    SB_LAUNCH_CHECK();
+  }
+}
+
 extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out) {
   SB_API_BEGIN
   require_init();
@@ -540,25 +1090,34 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
   // the descriptor arrays are copied to the device asynchronously: they live on the heap until the stream has consumed them
   // (cudaLaunchHostFunc below), so the call returns without a host synchronisation and the next row group's copy can be queued
   // on another stream while this one decodes
-  struct Keep {
-    std::vector<PageTask> tasks;
-    std::vector<ColTask> ctasks;
-  };
+  using Keep = ScanKeep;
   std::unique_ptr<Keep> keep(new Keep());
   std::vector<PageTask> &tasks = keep->tasks;
   std::vector<ColTask> &ctasks = keep->ctasks;
+  std::vector<StrColTask> &stasks = keep->stasks;
   ctasks.resize(ncols);
+  stasks.resize(ncols);
   std::vector<std::unique_ptr<Scratch>> temps;
+  auto scratch = [&](int64_t bytes) -> void * {
+    Scratch *s = new Scratch(bytes, st);
+    temps.emplace_back(s);
+    return s->ptr;
+  };
   sb_table *t = nullptr;
   try {
     for (int ci = 0; ci < ncols; ci++) {
       const sb_column_chunk &ch = chunks[ci];
       SB_REQUIRE(ch.data && ch.pages && ch.npages >= 0, "column chunk %d: null buffers", ci);
-      const int pw = phys_width_of(ch.physical_type);
+      const bool is_str = ch.physical_type == SB_PHYS_BYTE_ARRAY;
+      const int pw = is_str ? 0 : phys_width_of(ch.physical_type);
       const int ow = type_width(ch.type);
-      SB_REQUIRE(ow > 0, "column chunk %d: string columns are not supported by the GPU scan", ci);
-      SB_REQUIRE(pw == 0 ? ch.type == SB_BOOL : (pw == 8 ? ow == 8 : (ow <= 4 || ch.type == SB_DECIMAL64)), "column chunk %d: physical type %d cannot feed column type %d", ci,
-                 ch.physical_type, ch.type);
+      if (is_str) {
+        SB_REQUIRE(ch.type == SB_STRING, "column chunk %d: physical type BYTE_ARRAY decodes to SB_STRING only (got column type %d)", ci, ch.type);
+      } else {
+        SB_REQUIRE(ow > 0, "column chunk %d: string columns are decoded from physical type BYTE_ARRAY only", ci);
+        SB_REQUIRE(pw == 0 ? ch.type == SB_BOOL : (pw == 8 ? ow == 8 : (ow <= 4 || ch.type == SB_DECIMAL64)), "column chunk %d: physical type %d cannot feed column type %d", ci,
+                   ch.physical_type, ch.type);
+      }
       int64_t rows = 0;
       bool nullable = false;
       for (int p = 0; p < ch.npages; p++) {
@@ -574,6 +1133,66 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
       Scratch *dev = new Scratch(ch.data_bytes + 32, st);
       temps.emplace_back(dev);
       if (ch.data_bytes > 0) SB_CUDA(cudaMemcpyAsync(dev->ptr, ch.data, (size_t)ch.data_bytes, cudaMemcpyHostToDevice, st));
+      if (is_str) {
+        Column col;
+        col.type = SB_STRING;
+        col.length = nrows;
+        col.null_count = nullable ? -1 : 0;
+        col.offsets = buffer_alloc((nrows + 1) * 4 + 16, st);
+        if (nullable) col.validity = buffer_alloc(bitmap_alloc_bytes(nrows), st);
+        t->cols.push_back(col);
+        bool has_dba = false;
+        for (int p = 0; p < ch.npages; p++) has_dba |= ch.pages[p].encoding == SB_ENC_DELTA_BYTE_ARRAY;
+        StrColTask &sc = stasks[ci];
+        memset(&sc, 0, sizeof(sc));
+        sc.base = dev->as<uint8_t>();
+        sc.data_bytes = ch.data_bytes;
+        sc.rlen = (int32_t *)scratch(nrows * 4 + 16);
+        sc.rsrc = (int64_t *)scratch(nrows * 8 + 16);
+        sc.rpre = has_dba ? (int32_t *)scratch(nrows * 4 + 16) : nullptr;
+        if (nullable) {
+          sc.valid_bytes = (uint8_t *)scratch(nrows + 16);
+          sc.vlen = (int32_t *)scratch(nrows * 4 + 16);
+          sc.vsrc = (int64_t *)scratch(nrows * 8 + 16);
+          sc.vpre = has_dba ? (int32_t *)scratch(nrows * 4 + 16) : nullptr;
+        }
+        ctasks[ci].valid_bytes = sc.valid_bytes;
+        const bool has_dict = ch.dict_offset >= 0 && ch.dict_count >= 0;
+        if (has_dict) {   // every PLAIN byte array takes at least its 4-byte length
+          SB_REQUIRE(ch.dict_offset + (int64_t)ch.dict_count * 4 <= ch.data_bytes, "column chunk %d: dictionary overruns the chunk", ci);
+          sc.dict_offset = ch.dict_offset;
+          sc.dict_count = ch.dict_count;
+          sc.dict_len = (int32_t *)scratch((int64_t)ch.dict_count * 4 + 16);
+          sc.dict_src = (int64_t *)scratch((int64_t)ch.dict_count * 8 + 16);
+          if (ch.dict_count > 0) keep->dict_cols.push_back(ci);
+        }
+        int64_t row = 0;
+        for (int p = 0; p < ch.npages; p++) {
+          const sb_page &pg = ch.pages[p];
+          SB_REQUIRE(pg.values_offset >= 0 && pg.values_bytes >= 0 && pg.values_offset + pg.values_bytes <= ch.data_bytes && pg.def_offset >= 0 &&
+                         pg.def_offset + pg.def_bytes <= ch.data_bytes,
+                     "column chunk %d page %d: offsets outside the chunk", ci, p);
+          SB_REQUIRE(pg.encoding == SB_ENC_PLAIN || (pg.encoding == SB_ENC_RLE_DICTIONARY && has_dict) || pg.encoding == SB_ENC_DELTA_LENGTH_BYTE_ARRAY ||
+                         pg.encoding == SB_ENC_DELTA_BYTE_ARRAY,
+                     "column chunk %d page %d: encoding %d%s", ci, p, pg.encoding,
+                     pg.encoding == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : " is not supported for BYTE_ARRAY columns");
+          PageTask pt;
+          pt.values = dev->as<uint8_t>() + pg.values_offset;
+          pt.values_bytes = pg.values_bytes;
+          pt.def = pg.def_bytes > 0 ? dev->as<uint8_t>() + pg.def_offset : nullptr;
+          pt.def_bytes = pg.def_bytes;
+          pt.row_start = row;
+          pt.num_values = pg.num_values;
+          pt.encoding = pg.encoding;
+          pt.col = ci;
+          pt.pad = 0;
+          if (pg.num_values > 0) keep->str_pages.push_back(pt);
+          if (pg.num_values > 0 && pg.encoding == SB_ENC_DELTA_BYTE_ARRAY) keep->dba_pages.push_back(pt);
+          row += pg.num_values;
+        }
+        keep->str_cols.push_back(ci);
+        continue;
+      }
       Column col = column_alloc(ch.type, ch.scale, nrows, nullable, st);
       t->cols.push_back(col);
       ColTask &ct = ctasks[ci];
@@ -601,7 +1220,8 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
         const sb_page &pg = ch.pages[p];
         SB_REQUIRE(pg.values_offset >= 0 && pg.values_offset + pg.values_bytes <= ch.data_bytes && pg.def_offset + pg.def_bytes <= ch.data_bytes,
                    "column chunk %d page %d: offsets outside the chunk", ci, p);
-        SB_REQUIRE(pg.encoding == SB_ENC_PLAIN || (pg.encoding == SB_ENC_RLE_DICTIONARY && ct.dict) || (pg.encoding == SB_ENC_RLE_BOOLEAN && pw == 0),
+        SB_REQUIRE(pg.encoding == SB_ENC_PLAIN || (pg.encoding == SB_ENC_RLE_DICTIONARY && ct.dict) || (pg.encoding == SB_ENC_RLE_BOOLEAN && pw == 0) ||
+                       (pg.encoding == SB_ENC_DELTA_BINARY_PACKED && (ch.physical_type == SB_PHYS_INT32 || ch.physical_type == SB_PHYS_INT64)),
                    "column chunk %d page %d: encoding %d%s", ci, p, pg.encoding,
                    pg.encoding == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : " is not supported for this column");
         PageTask pt;
@@ -614,24 +1234,38 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
         pt.encoding = pg.encoding;
         pt.col = ci;
         pt.pad = 0;
-        tasks.push_back(pt);
+        (pg.encoding == SB_ENC_DELTA_BINARY_PACKED ? keep->delta_tasks : tasks).push_back(pt);
         row += pg.num_values;
       }
     }
-    if (!tasks.empty() && nrows > 0) {
-      Scratch d_pages((int64_t)tasks.size() * sizeof(PageTask), st), d_cols((int64_t)ncols * sizeof(ColTask), st);
-      SB_CUDA(cudaMemcpyAsync(d_pages.ptr, tasks.data(), tasks.size() * sizeof(PageTask), cudaMemcpyHostToDevice, st));
+    std::vector<PageTask> &dtasks = keep->delta_tasks;
+    const bool queued = nrows > 0 && (!tasks.empty() || !dtasks.empty());
+    if (queued) {
+      Scratch d_pages((int64_t)(tasks.size() + dtasks.size()) * sizeof(PageTask), st), d_cols((int64_t)ncols * sizeof(ColTask), st);
+      if (!tasks.empty()) SB_CUDA(cudaMemcpyAsync(d_pages.ptr, tasks.data(), tasks.size() * sizeof(PageTask), cudaMemcpyHostToDevice, st));
+      if (!dtasks.empty())
+        SB_CUDA(cudaMemcpyAsync(d_pages.as<PageTask>() + tasks.size(), dtasks.data(), dtasks.size() * sizeof(PageTask), cudaMemcpyHostToDevice, st));
       SB_CUDA(cudaMemcpyAsync(d_cols.ptr, ctasks.data(), (size_t)ncols * sizeof(ColTask), cudaMemcpyHostToDevice, st));
       {
         KernelTimer kt("scan_decode", st);
-        // enough blocks to fill the machine: pages of hybrid-encoded values are striped over `nparts` blocks each
-        int nparts = (int)((rt().num_sms * 6 + (int64_t)tasks.size() - 1) / (int64_t)tasks.size());
-        nparts = nparts < 1 ? 1 : (nparts > 16 ? 16 : nparts);
-        scan_decode_kernel<<<(unsigned)(tasks.size() * nparts), SCAN_THREADS, 0, st>>>(d_pages.as<PageTask>(), d_cols.as<ColTask>(), nparts);
-        SB_LAUNCH_CHECK();
+        if (!tasks.empty()) {
+          // enough blocks to fill the machine: pages of hybrid-encoded values are striped over `nparts` blocks each
+          int nparts = (int)((rt().num_sms * 6 + (int64_t)tasks.size() - 1) / (int64_t)tasks.size());
+          nparts = nparts < 1 ? 1 : (nparts > 16 ? 16 : nparts);
+          scan_decode_kernel<<<(unsigned)(tasks.size() * nparts), SCAN_THREADS, 0, st>>>(d_pages.as<PageTask>(), d_cols.as<ColTask>(), nparts);
+          SB_LAUNCH_CHECK();
+        }
+        if (!dtasks.empty()) {
+          scan_delta_kernel<<<(unsigned)dtasks.size(), SCAN_THREADS, 0, st>>>(d_pages.as<PageTask>() + tasks.size(), d_cols.as<ColTask>());
+          SB_LAUNCH_CHECK();
+        }
       }
-      for (int ci = 0; ci < ncols; ci++)
-        if (ctasks[ci].valid_bytes) bytes_to_bitmap(ctasks[ci].valid_bytes, nrows, (uint32_t *)t->cols[ci].validity->ptr, st);
+    }
+    if (!keep->str_cols.empty()) decode_strings(*keep, t, nrows, st);
+    if (queued || !keep->str_cols.empty()) {
+      if (nrows > 0)
+        for (int ci = 0; ci < ncols; ci++)
+          if (ctasks[ci].valid_bytes) bytes_to_bitmap(ctasks[ci].valid_bytes, nrows, (uint32_t *)t->cols[ci].validity->ptr, st);
       Keep *raw = keep.release();
       if (cudaLaunchHostFunc(st, [](void *p) { delete (Keep *)p; }, raw) != cudaSuccess) {
         cudaGetLastError();

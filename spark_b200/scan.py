@@ -20,10 +20,17 @@ from .columnar import ColumnarBatch, _h
 from .execution import SparkPlan
 
 _PHYS = {"BOOLEAN": capi.SB_PHYS["BOOLEAN"], "INT32": capi.SB_PHYS["INT32"], "INT64": capi.SB_PHYS["INT64"],
-         "FLOAT": capi.SB_PHYS["FLOAT"], "DOUBLE": capi.SB_PHYS["DOUBLE"]}
+         "FLOAT": capi.SB_PHYS["FLOAT"], "DOUBLE": capi.SB_PHYS["DOUBLE"], "BYTE_ARRAY": capi.SB_PHYS["BYTE_ARRAY"]}
+
+
+def _is_bytes(arrow_type):
+    return (pa.types.is_string(arrow_type) or pa.types.is_large_string(arrow_type) or pa.types.is_binary(arrow_type)
+            or pa.types.is_large_binary(arrow_type))
 
 
 def _sb_type(arrow_type):
+    if _is_bytes(arrow_type):      # BYTE_ARRAY -> int32 offsets + byte arena; a binary column comes back as binary
+        return capi.SB_STRING, 0
     if pa.types.is_decimal(arrow_type):
         if arrow_type.precision > 18:
             raise capi.SparkB200Error(5, "decimal precision %d > 18 is not supported by the GPU scan" % arrow_type.precision)
@@ -98,6 +105,8 @@ class ParquetScanExec(SparkPlan):
                 raise capi.SparkB200Error(5, "column %s is %s-compressed; the GPU scan reads uncompressed pages" % (f.name, cm.compression))
             if cm.physical_type not in _PHYS:
                 raise capi.SparkB200Error(5, "column %s: physical type %s is not supported by the GPU scan" % (f.name, cm.physical_type))
+            if (cm.physical_type == "BYTE_ARRAY") != _is_bytes(f.type):
+                raise capi.SparkB200Error(5, "column %s: physical type %s with Arrow type %s is not supported by the GPU scan" % (f.name, cm.physical_type, f.type))
             start = cm.dictionary_page_offset if cm.has_dictionary_page and cm.dictionary_page_offset else cm.data_page_offset
             start = min(start, cm.data_page_offset)
             buf = self._bytes[start:start + cm.total_compressed_size]
