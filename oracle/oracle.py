@@ -108,11 +108,14 @@ _NP = {SO_BOOL: np.uint8, SO_INT8: np.int8, SO_INT16: np.int16, SO_INT32: np.int
 class Col:
     """One column held as numpy values + numpy bool validity (None = all valid)."""
 
-    def __init__(self, so_type, values, valid=None, offsets=None):
+    def __init__(self, so_type, values, valid=None, offsets=None, arrow_type=None):
         self.type = so_type
         self.values = np.ascontiguousarray(values)
         self.valid = None if valid is None or bool(np.all(valid)) else np.ascontiguousarray(valid, dtype=bool)
         self.offsets = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.int32)
+        # decimal(p, s) / timestamp unit of the values: set by from_arrow, kept by take(), restored by to_arrow().  Cols built from
+        # the C oracle's outputs have none: a decimal or timestamp result comes back as plain int64
+        self.arrow_type = arrow_type
         self._keep = []
 
     def __len__(self):
@@ -126,12 +129,19 @@ class Col:
         if pa.types.is_timestamp(t):
             so = SO_TIMESTAMP
         elif pa.types.is_decimal(t):
-            raise NotImplementedError("decimal128 columns: pass the unscaled int64 values")
+            if t.precision > 18:
+                raise NotImplementedError("decimal(p > 18) columns: only decimal(p <= 18) is a long of unscaled values")
+            so = SO_DECIMAL64
         else:
             so = _ARROW2SO[t]
         valid = None
         if arr.null_count:
             valid = np.asarray(arr.is_valid())
+        if so == SO_DECIMAL64:   # Decimal.scala: precision <= 18 is held as the unscaled long (low half of Arrow's 16 bytes)
+            n = len(arr)
+            raw = np.frombuffer(pa.concat_arrays([arr]).buffers()[1], dtype=np.int64, count=2 * n).reshape(n, 2)
+            vals = np.where(valid, raw[:, 0], 0) if valid is not None else raw[:, 0]
+            return Col(so, vals.astype(np.int64), valid, arrow_type=t)
         if so == SO_STRING:
             n = len(arr)
             arr = pa.concat_arrays([arr]) if arr.offset else arr
@@ -147,7 +157,7 @@ class Col:
             vals = np.asarray(arr.cast(pa.int64()).fill_null(0))
         else:
             vals = np.asarray(arr.fill_null(0))
-        return Col(so, vals.astype(_NP[so], copy=False), valid)
+        return Col(so, vals.astype(_NP[so], copy=False), valid, arrow_type=t if so == SO_TIMESTAMP else None)
 
     def to_arrow(self):
         mask = None if self.valid is None else ~self.valid
@@ -160,9 +170,18 @@ class Col:
                                                           pa.py_buffer(self.values.tobytes())])
         if self.type == SO_BOOL:
             return pa.array(self.values.astype(bool), mask=mask)
+        if self.type == SO_DECIMAL64 and self.arrow_type is not None:
+            n = len(self.values)
+            wide = np.empty((n, 2), np.int64)
+            wide[:, 0] = self.values
+            wide[:, 1] = self.values >> 63            # sign extension to Arrow's 16-byte two's complement
+            vb = None if self.valid is None else pa.py_buffer(np.packbits(self.valid, bitorder="little").tobytes())
+            return pa.Array.from_buffers(self.arrow_type, n, [vb, pa.py_buffer(wide.tobytes())])
         a = pa.array(self.values, mask=mask)
         if self.type == SO_DATE32:
             a = a.cast(pa.date32())
+        elif self.type == SO_TIMESTAMP and self.arrow_type is not None:
+            a = a.cast(self.arrow_type)
         return a
 
     def bitmap(self):
@@ -201,7 +220,7 @@ class Col:
         else:
             vals = self.values[safe]
             valid = (np.ones(len(idx), bool) if self.valid is None else self.valid[safe]) & ~neg
-        return Col(self.type, vals, valid)
+        return Col(self.type, vals, valid, arrow_type=self.arrow_type)
 
 
 def _cols(table, names):
@@ -497,6 +516,19 @@ def project(table, named_exprs):
 
 
 # --------------------------------------------------------------------------- hash aggregate
+def normalize_floats(col: Col) -> Col:
+    """NormalizeNaNAndZero (sql/catalyst/.../optimizer/NormalizeFloatingNumbers.scala:180-199): -0.0 -> 0.0 and every NaN -> the
+    canonical Float.NaN / Double.NaN (0x7fc00000 / 0x7ff8000000000000).  The aggregation strategy applies it to the grouping
+    expressions (sql/core/.../execution/SparkStrategies.scala:736-745), so a group key comes out normalised."""
+    if col.type not in (SO_FLOAT32, SO_FLOAT64):
+        return col
+    v = col.values.copy()
+    with np.errstate(invalid="ignore"):
+        v[v == 0] = 0.0
+    v[np.isnan(v)] = np.nan      # numpy's nan is the canonical quiet NaN in both widths
+    return Col(col.type, v, col.valid)
+
+
 def _group(table, key_cols):
     n = table.num_rows
     cols = _cols(table, key_cols)
@@ -525,7 +557,7 @@ def hash_aggregate(table, key_cols, aggs, mode="complete"):
     n = table.num_rows
     out_names, out_cols = [], []
     for k in key_cols:
-        out_names.append(k); out_cols.append(Col.from_arrow(table.column(k)).take(first))
+        out_names.append(k); out_cols.append(normalize_floats(Col.from_arrow(table.column(k)).take(first)))
     gp = gid.ctypes.data
 
     def sum_of(col):
