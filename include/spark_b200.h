@@ -212,10 +212,48 @@ typedef struct sb_column_chunk {
  * continue the previous page's last value, PARQUET-246) -> SB_ERR_UNSUPPORTED. */
 int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int32_t max_def_level, sb_page *out_pages, int32_t pages_cap,
                            int32_t *out_npages, int64_t *out_dict_offset, int32_t *out_dict_count);
-/* one H2D copy per column chunk, then one decode kernel (a block per page).  A call with only fixed-width columns does not
+/* uncompressed pages only (see sb_scan_decode_compressed): one H2D copy per column chunk, then one decode kernel (a block per page). A call with only fixed-width columns does not
  * synchronise the stream.  A call that decodes SB_STRING columns (physical BYTE_ARRAY) synchronises it once, to read back the
  * arena sizes of all of them together; an arena above 2^31 - 1 bytes is SB_ERR_UNSUPPORTED. */
 int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out);
+
+/* Compressed column chunks.  The host walks the page headers (Parquet never compresses them) into spans; the device does
+ * everything that needs the page bodies. */
+#define SB_CODEC_UNCOMPRESSED 0     /* parquet.thrift CompressionCodec */
+#define SB_CODEC_SNAPPY 1           /* a raw Snappy block per page body (no framing), as parquet-mr and parquet-cpp write it */
+
+typedef struct sb_page_span {       /* one page of a chunk as it lies in the file; offsets relative to the chunk */
+  int32_t page_type;                /* 0 DATA_PAGE, 2 DICTIONARY_PAGE, 3 DATA_PAGE_V2 */
+  int32_t encoding;                 /* SB_ENC_* (dictionary page: SB_ENC_PLAIN) */
+  int32_t num_values;
+  int32_t levels_bytes;             /* V2: repetition + definition level bytes, stored uncompressed in front of the values */
+  int64_t body_offset;              /* first byte after the page header */
+  int32_t compressed_bytes, uncompressed_bytes;
+  int32_t values_compressed;        /* 0: UNCOMPRESSED chunk, or a V2 page with is_compressed = false */
+  int32_t header_bytes;             /* the page header, which starts at body_offset - header_bytes */
+} sb_page_span;
+
+typedef struct sb_compressed_chunk {
+  int32_t type, scale, physical_type, codec;   /* codec: SB_CODEC_* */
+  int32_t max_def_level, npages;
+  const uint8_t *data;              /* HOST bytes of the chunk as they lie in the file, headers included */
+  int64_t data_bytes;
+  const sb_page_span *spans;        /* from sb_parquet_page_spans, the dictionary page included */
+} sb_compressed_chunk;
+
+/* host only (no device): the spans of every dictionary and data page of a chunk.  Checks that each body lies inside the chunk,
+ * that the level bytes fit the page, that a dictionary page is PLAIN and that there are no repetition levels.  Whether a page is
+ * compressed comes from the codec (the footer's), not from its two sizes.  A codec other than SB_CODEC_UNCOMPRESSED or
+ * SB_CODEC_SNAPPY (GZIP, LZO, BROTLI, LZ4, ZSTD, LZ4_RAW) -> SB_ERR_UNSUPPORTED. */
+int sb_parquet_page_spans(const uint8_t *chunk, int64_t nbytes, int32_t codec, int32_t max_def_level, sb_page_span *out, int32_t cap,
+                          int32_t *out_n);
+/* sb_scan_decode for chunks whose pages may be compressed (a chunk may mix V1, V2 and dictionary pages).  One H2D copy per chunk,
+ * then scan_snappy decompresses every page of the call into one device image per chunk and scan_resolve_pages reads each page's
+ * level length and values header from it.  The call synchronises the stream once for those records: a malformed Snappy stream
+ * is SB_ERR_INVALID naming the page, and the page checks of sb_parquet_chunk_pages follow with the same messages.  The decode
+ * itself is sb_scan_decode's over the images (one more synchronisation when string columns are decoded). */
+int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out);
+
 /* write-side twin (tests, bench.py): one NULL-free fixed-width column -> a column chunk on the device (out_chunk: one SB_INT8
  * column of bytes) + page descriptors on the host.  dictionary: one-column table of the distinct values in ascending order,
  * or NULL for PLAIN pages. */

@@ -115,4 +115,12 @@ public final class Native {
    *  parquetChunkPages returned it */
   public static native long scanDecode(int[] types, int[] scales, int[] physicalTypes, long[] chunkAddresses, long[] chunkBytes,
                                        long[][] pageTables, long stream);
+  /** spans of the pages of a chunk whose pages may be compressed (codec: parquet.thrift CompressionCodec, UNCOMPRESSED or SNAPPY):
+   *  rows of {pageType, encoding, numValues, levelsBytes, bodyOffset, compressedBytes, uncompressedBytes, valuesCompressed,
+   *  headerBytes} */
+  public static native long[] parquetPageSpans(long chunkAddress, long chunkBytes, int codec, int maxDefLevel);
+  /** scanDecode for chunks whose pages may be SNAPPY-compressed: one entry per column, its span table as parquetPageSpans
+   *  returned it */
+  public static native long scanDecodeCompressed(int[] types, int[] scales, int[] physicalTypes, int[] codecs, int[] maxDefLevels,
+                                                 long[] chunkAddresses, long[] chunkBytes, long[][] spanTables, long stream);
 }

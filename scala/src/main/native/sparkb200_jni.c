@@ -625,6 +625,90 @@ NATIVE(jlong, scanDecode)(JNIEnv *env, jclass c, jintArray types, jintArray scal
   return (jlong)(intptr_t)out;
 }
 
+/* span tables travel as long[9 * nspans]: rows of {page_type, encoding, num_values, levels_bytes, body_offset, compressed_bytes,
+ * uncompressed_bytes, values_compressed, header_bytes} */
+#define SB_JNI_SPAN_WORDS 9
+NATIVE(jlongArray, parquetPageSpans)(JNIEnv *env, jclass c, jlong chunk, jlong nbytes, jint codec, jint maxDef) {
+  sb_page_span *spans = (sb_page_span *)calloc(SB_JNI_MAX_PAGES, sizeof(sb_page_span));
+  int32_t n = 0;
+  int rc = sb_parquet_page_spans((const uint8_t *)(intptr_t)chunk, nbytes, codec, maxDef, spans, SB_JNI_MAX_PAGES, &n);
+  jlongArray out = NULL;
+  if (rc == SB_OK) {
+    jlong *flat = (jlong *)calloc((size_t)(n > 0 ? n : 1) * SB_JNI_SPAN_WORDS, sizeof(jlong));
+    for (int32_t i = 0; i < n; i++) {
+      jlong *w = flat + (size_t)i * SB_JNI_SPAN_WORDS;
+      w[0] = spans[i].page_type;
+      w[1] = spans[i].encoding;
+      w[2] = spans[i].num_values;
+      w[3] = spans[i].levels_bytes;
+      w[4] = spans[i].body_offset;
+      w[5] = spans[i].compressed_bytes;
+      w[6] = spans[i].uncompressed_bytes;
+      w[7] = spans[i].values_compressed;
+      w[8] = spans[i].header_bytes;
+    }
+    out = (*env)->NewLongArray(env, n * SB_JNI_SPAN_WORDS);
+    (*env)->SetLongArrayRegion(env, out, 0, n * SB_JNI_SPAN_WORDS, flat);
+    free(flat);
+  }
+  free(spans);
+  throw_if(env, rc);
+  return out;
+}
+NATIVE(jlong, scanDecodeCompressed)(JNIEnv *env, jclass c, jintArray types, jintArray scales, jintArray phys, jintArray codecs, jintArray maxDefs,
+                                    jlongArray addrs, jlongArray sizes, jobjectArray spanTables, jlong stream) {
+  jsize ncols = (*env)->GetArrayLength(env, types);
+  jint *ty = (*env)->GetIntArrayElements(env, types, NULL), *sc = (*env)->GetIntArrayElements(env, scales, NULL);
+  jint *ph = (*env)->GetIntArrayElements(env, phys, NULL), *co = (*env)->GetIntArrayElements(env, codecs, NULL);
+  jint *md = (*env)->GetIntArrayElements(env, maxDefs, NULL);
+  jlong *ad = (*env)->GetLongArrayElements(env, addrs, NULL), *sz = (*env)->GetLongArrayElements(env, sizes, NULL);
+  sb_compressed_chunk *chunks = (sb_compressed_chunk *)calloc((size_t)(ncols ? ncols : 1), sizeof(sb_compressed_chunk));
+  sb_page_span **owned = (sb_page_span **)calloc((size_t)(ncols ? ncols : 1), sizeof(sb_page_span *));
+  for (jsize i = 0; i < ncols; i++) {
+    jlongArray st = (jlongArray)(*env)->GetObjectArrayElement(env, spanTables, i);
+    jsize words = (*env)->GetArrayLength(env, st);
+    jlong *flat = (*env)->GetLongArrayElements(env, st, NULL);
+    int32_t n = (int32_t)(words / SB_JNI_SPAN_WORDS);
+    owned[i] = (sb_page_span *)calloc((size_t)(n > 0 ? n : 1), sizeof(sb_page_span));
+    for (int32_t p = 0; p < n; p++) {
+      const jlong *w = flat + (size_t)p * SB_JNI_SPAN_WORDS;
+      owned[i][p].page_type = (int32_t)w[0];
+      owned[i][p].encoding = (int32_t)w[1];
+      owned[i][p].num_values = (int32_t)w[2];
+      owned[i][p].levels_bytes = (int32_t)w[3];
+      owned[i][p].body_offset = w[4];
+      owned[i][p].compressed_bytes = (int32_t)w[5];
+      owned[i][p].uncompressed_bytes = (int32_t)w[6];
+      owned[i][p].values_compressed = (int32_t)w[7];
+      owned[i][p].header_bytes = (int32_t)w[8];
+    }
+    chunks[i].type = ty[i];
+    chunks[i].scale = sc[i];
+    chunks[i].physical_type = ph[i];
+    chunks[i].codec = co[i];
+    chunks[i].max_def_level = md[i];
+    chunks[i].npages = n;
+    chunks[i].data = (const uint8_t *)(intptr_t)ad[i];
+    chunks[i].data_bytes = sz[i];
+    chunks[i].spans = owned[i];
+    (*env)->ReleaseLongArrayElements(env, st, flat, JNI_ABORT);
+  }
+  sb_table *out = NULL;
+  int rc = sb_scan_decode_compressed(chunks, ncols, STR(stream), &out);
+  for (jsize i = 0; i < ncols; i++) free(owned[i]);
+  free(owned);
+  free(chunks);
+  (*env)->ReleaseLongArrayElements(env, sizes, sz, JNI_ABORT);
+  (*env)->ReleaseLongArrayElements(env, addrs, ad, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, maxDefs, md, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, codecs, co, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, phys, ph, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, scales, sc, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, types, ty, JNI_ABORT);
+  throw_if(env, rc);
+  return (jlong)(intptr_t)out;
+}
+
 NATIVE(jlongArray, exchangeCounts)(JNIEnv *env, jclass c, jlongArray partOffsets, jint n, jint nranks, jlong stream) {
   jlong *in = (*env)->GetLongArrayElements(env, partOffsets, NULL);
   const jsize total = (jsize)n * (nranks > 0 ? nranks : 1);

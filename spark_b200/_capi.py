@@ -46,6 +46,21 @@ class sb_column_chunk(C.Structure):
                 ("data_bytes", C.c_int64), ("pages", C.POINTER(sb_page)), ("dict_offset", C.c_int64), ("dict_count", C.c_int32), ("pad", C.c_int32)]
 
 
+class sb_page_span(C.Structure):
+    _fields_ = [("page_type", C.c_int32), ("encoding", C.c_int32), ("num_values", C.c_int32), ("levels_bytes", C.c_int32),
+                ("body_offset", C.c_int64), ("compressed_bytes", C.c_int32), ("uncompressed_bytes", C.c_int32),
+                ("values_compressed", C.c_int32), ("header_bytes", C.c_int32)]
+
+
+class sb_compressed_chunk(C.Structure):
+    _fields_ = [("type", C.c_int32), ("scale", C.c_int32), ("physical_type", C.c_int32), ("codec", C.c_int32),
+                ("max_def_level", C.c_int32), ("npages", C.c_int32), ("data", C.c_void_p), ("data_bytes", C.c_int64),
+                ("spans", C.POINTER(sb_page_span))]
+
+
+# parquet.thrift CompressionCodec; the GPU scan decodes UNCOMPRESSED and SNAPPY
+SB_CODEC = dict(UNCOMPRESSED=0, SNAPPY=1, GZIP=2, LZO=3, BROTLI=4, LZ4=5, ZSTD=6, LZ4_RAW=7)
+
 SB_ENC_PLAIN, SB_ENC_RLE_DICTIONARY, SB_ENC_RLE_BOOLEAN = 0, 1, 2
 SB_ENC_DELTA_BINARY_PACKED, SB_ENC_DELTA_LENGTH_BYTE_ARRAY, SB_ENC_DELTA_BYTE_ARRAY = 3, 4, 5
 SB_PHYS = dict(BOOLEAN=0, INT32=1, INT64=2, FLOAT=4, DOUBLE=5, BYTE_ARRAY=6)
@@ -131,6 +146,8 @@ _SIGNATURES = {
     "sb_window": [_p, C.POINTER(C.c_int32), _i32, C.POINTER(sb_sort_order), _i32, C.POINTER(sb_window_spec), _i32, _p, _pp], "sb_expand": [_p, _p, _i32, _i32, _p, _pp],
     "sb_parquet_chunk_pages": [_p, _i64, _i32, C.POINTER(sb_page), _i32, C.POINTER(_i32), C.POINTER(_i64), C.POINTER(_i32)],
     "sb_scan_decode": [C.POINTER(sb_column_chunk), _i32, _p, _pp],
+    "sb_parquet_page_spans": [_p, _i64, _i32, _i32, C.POINTER(sb_page_span), _i32, C.POINTER(_i32)],
+    "sb_scan_decode_compressed": [C.POINTER(sb_compressed_chunk), _i32, _p, _pp],
     "sb_scan_encode": [_p, _i32, _p, _i64, _p, _pp, C.POINTER(sb_page), _i32, C.POINTER(_i32), C.POINTER(_i64), C.POINTER(_i32)],
     "sb_filter_project": [_p, C.POINTER(sb_expr), C.POINTER(sb_expr), _i32, _p, _pp],
     "sb_partition_ids": [_p, C.POINTER(_i32), _i32, _i32, _p, _p],

@@ -13,8 +13,8 @@
 // Supported: physical types BOOLEAN / INT32 / INT64 / FLOAT / DOUBLE, and BYTE_ARRAY decoded to SB_STRING; encodings PLAIN,
 // RLE_DICTIONARY (= PLAIN_DICTIONARY: bit-width byte + hybrid runs over a PLAIN dictionary page), DELTA_BINARY_PACKED (INT32 /
 // INT64), DELTA_LENGTH_BYTE_ARRAY and DELTA_BYTE_ARRAY (BYTE_ARRAY); data pages V1 (levels length-prefixed in front of the
-// values) and V2 (levels in their own section); flat schemas (max definition level <= 1, no repetition); uncompressed pages
-// (the codec is the file writer's choice; decompression is not part of this path).  FIXED_LEN_BYTE_ARRAY, INT96 and
+// values) and V2 (levels in their own section); flat schemas (max definition level <= 1, no repetition); uncompressed pages, or
+// SNAPPY pages through sb_scan_decode_compressed (decompressed on the device by snappy.cu).  FIXED_LEN_BYTE_ARRAY, INT96 and
 // BYTE_STREAM_SPLIT are rejected with SB_ERR_UNSUPPORTED rather than decoded on the CPU.
 //
 // Kernel: one 256-thread block per page.  (1) definition levels -> one validity byte per row; (2) values -> dense value
@@ -27,6 +27,7 @@
 #include <memory>
 #include "common.cuh"
 #include "primitives.cuh"
+#include "snappy.cuh"
 
 namespace sb {
 
@@ -930,6 +931,55 @@ void check_delta_header(const uint8_t *p, int64_t nbytes, int32_t enc, int64_t p
     fail(SB_ERR_UNSUPPORTED, "page %d (byte %lld of the column chunk): DELTA_BYTE_ARRAY page starts with prefix length %lld; continuing the "
          "previous page's value (PARQUET-246) is not supported", page, (long long)page_pos, (long long)first);
 }
+
+// SB_ENC_* of a data page's Parquet encoding
+int32_t page_encoding(int32_t parquet_encoding) {
+  switch (parquet_encoding) {
+    case 0: return SB_ENC_PLAIN;
+    case 2: case 8: return SB_ENC_RLE_DICTIONARY;
+    case 3: return SB_ENC_RLE_BOOLEAN;   // only BOOLEAN columns may use it (checked in sb_scan_decode)
+    case 5: return SB_ENC_DELTA_BINARY_PACKED;
+    case 6: return SB_ENC_DELTA_LENGTH_BYTE_ARRAY;
+    case 7: return SB_ENC_DELTA_BYTE_ARRAY;
+  }
+  fail(SB_ERR_UNSUPPORTED, "Parquet value encoding %d is not supported (PLAIN, RLE_DICTIONARY and the DELTA encodings are)", parquet_encoding);
+}
+
+// the checks a data page's header alone decides
+void check_data_page_header(const PageHeader &h, int32_t max_def_level) {
+  if (h.type == 0) {
+    if (max_def_level > 0) SB_REQUIRE(h.def_enc == 3, "definition levels must be RLE encoded (got %d)", h.def_enc);
+  } else {
+    SB_REQUIRE(h.rep_len == 0, "repeated fields are not supported");
+  }
+}
+
+// Levels and values of one data page whose body (as decoded) is [body, body + body_bytes) of the chunk: a V1 page of an optional
+// column starts with the 4-byte length of its definition levels (`len4`; nullptr when the body is shorter), a V2 page gives the
+// length in its header.  Both page walkers call it (and then check_delta_header on the values), so a page is refused with the same
+// message whether or not it was compressed.
+void data_page_sections(sb_page &pg, bool v1, int32_t max_def_level, int32_t v2_def_len, int64_t body, int64_t body_bytes, const uint8_t *len4) {
+  int64_t vpos = body;
+  const int64_t vend = body + body_bytes;
+  if (v1) {
+    if (max_def_level > 0) {   // [4-byte length][RLE definition levels]
+      SB_REQUIRE(len4 != nullptr, "truncated definition levels");
+      const uint32_t len = (uint32_t)len4[0] | ((uint32_t)len4[1] << 8) | ((uint32_t)len4[2] << 16) | ((uint32_t)len4[3] << 24);
+      pg.def_offset = vpos + 4;
+      pg.def_bytes = len;
+      vpos += 4 + (int64_t)len;
+    }
+  } else {
+    if (v2_def_len > 0) {
+      pg.def_offset = vpos;
+      pg.def_bytes = v2_def_len;
+    }
+    vpos += v2_def_len;
+  }
+  SB_REQUIRE(vpos <= vend, "Parquet page levels overrun the page");
+  pg.values_offset = vpos;
+  pg.values_bytes = vend - vpos;
+}
 }  // namespace
 
 // Host only (no device needed): walks the pages of one column chunk as it lies in a Parquet file (the byte range
@@ -961,40 +1011,70 @@ extern "C" int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int3
       SB_REQUIRE(np < pages_cap, "more than %d pages in the column chunk", pages_cap);
       sb_page &pg = out_pages[np++];
       memset(&pg, 0, sizeof(pg));
-      if (h.encoding == 0) pg.encoding = SB_ENC_PLAIN;
-      else if (h.encoding == 2 || h.encoding == 8) pg.encoding = SB_ENC_RLE_DICTIONARY;
-      else if (h.encoding == 3) pg.encoding = SB_ENC_RLE_BOOLEAN;   // only BOOLEAN columns may use it (checked in sb_scan_decode)
-      else if (h.encoding == 5) pg.encoding = SB_ENC_DELTA_BINARY_PACKED;
-      else if (h.encoding == 6) pg.encoding = SB_ENC_DELTA_LENGTH_BYTE_ARRAY;
-      else if (h.encoding == 7) pg.encoding = SB_ENC_DELTA_BYTE_ARRAY;
-      else fail(SB_ERR_UNSUPPORTED, "Parquet value encoding %d is not supported (PLAIN, RLE_DICTIONARY and the DELTA encodings are)", h.encoding);
+      pg.encoding = page_encoding(h.encoding);
       pg.num_values = h.num_values;
-      int64_t vpos = body, vend = body + h.compressed;
-      if (h.type == 0) {
-        if (max_def_level > 0) {   // [4-byte length][RLE definition levels]
-          SB_REQUIRE(h.def_enc == 3, "definition levels must be RLE encoded (got %d)", h.def_enc);
-          SB_REQUIRE(vpos + 4 <= vend, "truncated definition levels");
-          const uint32_t len = (uint32_t)chunk[vpos] | ((uint32_t)chunk[vpos + 1] << 8) | ((uint32_t)chunk[vpos + 2] << 16) | ((uint32_t)chunk[vpos + 3] << 24);
-          pg.def_offset = vpos + 4;
-          pg.def_bytes = len;
-          vpos += 4 + (int64_t)len;
-        }
-      } else {
-        SB_REQUIRE(h.rep_len == 0, "repeated fields are not supported");
-        if (h.def_len > 0) {
-          pg.def_offset = vpos;
-          pg.def_bytes = h.def_len;
-        }
-        vpos += h.def_len;
-      }
-      SB_REQUIRE(vpos <= vend, "Parquet page levels overrun the page");
-      pg.values_offset = vpos;
-      pg.values_bytes = vend - vpos;
-      if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED) check_delta_header(chunk + vpos, vend - vpos, pg.encoding, h.num_values, np - 1, pos);
+      check_data_page_header(h, max_def_level);
+      data_page_sections(pg, h.type == 0, max_def_level, h.def_len, body, h.compressed, h.compressed >= 4 ? chunk + body : nullptr);
+      if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED) check_delta_header(chunk + pg.values_offset, pg.values_bytes, pg.encoding, h.num_values, np - 1, pos);
     }   // INDEX_PAGE and unknown page types are skipped
     pos = body + h.compressed;
   }
   *out_npages = np;
+  SB_API_END
+}
+
+static void require_codec(int32_t codec) {
+  static const char *const names[] = {"UNCOMPRESSED", "SNAPPY", "GZIP", "LZO", "BROTLI", "LZ4", "ZSTD", "LZ4_RAW"};
+  if (codec == SB_CODEC_UNCOMPRESSED || codec == SB_CODEC_SNAPPY) return;
+  if (codec > 0 && codec < 8) fail(SB_ERR_UNSUPPORTED, "Parquet compression codec %s is not supported by the GPU scan (UNCOMPRESSED and SNAPPY are)", names[codec]);
+  fail(SB_ERR_UNSUPPORTED, "Parquet compression codec %d is not supported by the GPU scan (UNCOMPRESSED and SNAPPY are)", codec);
+}
+
+// Host only: the spans of a chunk whose pages may be compressed.  Unlike sb_parquet_chunk_pages it never looks inside a body:
+// whether a page is compressed comes from the footer's codec (a Snappy page may compress to exactly its own size, and tiny
+// pages grow), and the levels and DELTA headers are checked once the device has decoded the bodies.
+extern "C" int sb_parquet_page_spans(const uint8_t *chunk, int64_t nbytes, int32_t codec, int32_t max_def_level, sb_page_span *out, int32_t cap,
+                                     int32_t *out_n) {
+  SB_API_BEGIN
+  SB_REQUIRE(chunk && out && out_n && nbytes >= 0, "null argument");
+  require_codec(codec);
+  SB_REQUIRE(max_def_level == 0 || max_def_level == 1, "nested schemas are not supported (max definition level %d)", max_def_level);
+  int32_t n = 0;
+  int64_t pos = 0;
+  while (pos < nbytes) {
+    Thrift t{chunk + pos, chunk + nbytes};
+    PageHeader h;
+    if (!read_page_header(t, h)) fail(SB_ERR_INVALID, "malformed Parquet page header at byte %lld of the column chunk", (long long)pos);
+    const int64_t body = t.p - chunk;
+    SB_REQUIRE(h.compressed >= 0 && h.uncompressed >= 0 && body + h.compressed <= nbytes, "Parquet page at byte %lld overruns the column chunk",
+               (long long)pos);
+    if (h.type == 0 || h.type == 2 || h.type == 3) {
+      SB_REQUIRE(n < cap, "more than %d pages in the column chunk", cap);
+      sb_page_span &sp = out[n++];
+      memset(&sp, 0, sizeof(sp));
+      sp.page_type = h.type;
+      sp.num_values = h.num_values;
+      sp.body_offset = body;
+      sp.header_bytes = (int32_t)(body - pos);
+      sp.compressed_bytes = h.compressed;
+      sp.uncompressed_bytes = h.uncompressed;
+      sp.values_compressed = codec != SB_CODEC_UNCOMPRESSED && !(h.is_v2 && !h.v2_compressed);
+      if (h.type == 2) {
+        SB_REQUIRE(h.encoding == 0 || h.encoding == 2, "dictionary page encoding %d is not PLAIN", h.encoding);
+        sp.encoding = SB_ENC_PLAIN;
+      } else {
+        sp.encoding = page_encoding(h.encoding);
+        check_data_page_header(h, max_def_level);
+        if (h.type == 3) sp.levels_bytes = h.def_len;
+      }
+      SB_REQUIRE(sp.levels_bytes >= 0 && sp.levels_bytes <= h.uncompressed && sp.levels_bytes <= h.compressed, "Parquet page levels overrun the page");
+      if (!sp.values_compressed)
+        SB_REQUIRE(h.compressed == h.uncompressed, "uncompressed Parquet page at byte %lld: %d stored bytes for %d", (long long)pos, h.compressed,
+                   h.uncompressed);
+    }   // INDEX_PAGE and unknown page types are skipped
+    pos = body + h.compressed;
+  }
+  *out_n = n;
   SB_API_END
 }
 
@@ -1081,11 +1161,11 @@ static void decode_strings(ScanKeep &k, sb_table *t, int64_t nrows, cudaStream_t
   }
 }
 
-extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out) {
-  SB_API_BEGIN
-  require_init();
-  SB_REQUIRE(chunks && out && ncols > 0, "null argument");
-  cudaStream_t st = stream_of(s);
+// Descriptors and launches of one decode call.  device_bytes(chunk, temps) returns where chunk's bytes (the offsets of its pages
+// and dictionary) lie on the device; it is called once per chunk, in order, and may queue the chunk's copy and keep its buffer
+// in temps.  Returns the table; the caller owns it.
+template <class DeviceBytes>
+static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols, cudaStream_t st, DeviceBytes device_bytes) {
   int64_t nrows = -1;
   // the descriptor arrays are copied to the device asynchronously: they live on the heap until the stream has consumed them
   // (cudaLaunchHostFunc below), so the call returns without a host synchronisation and the next row group's copy can be queued
@@ -1129,10 +1209,7 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
         t = table_new(nrows);
       }
       SB_REQUIRE(rows == nrows, "column chunk %d has %lld rows, chunk 0 has %lld", ci, (long long)rows, (long long)nrows);
-      // the encoded bytes cross PCIe once, as they lie in the file
-      Scratch *dev = new Scratch(ch.data_bytes + 32, st);
-      temps.emplace_back(dev);
-      if (ch.data_bytes > 0) SB_CUDA(cudaMemcpyAsync(dev->ptr, ch.data, (size_t)ch.data_bytes, cudaMemcpyHostToDevice, st));
+      const uint8_t *dev = device_bytes(ch, temps);
       if (is_str) {
         Column col;
         col.type = SB_STRING;
@@ -1145,7 +1222,7 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
         for (int p = 0; p < ch.npages; p++) has_dba |= ch.pages[p].encoding == SB_ENC_DELTA_BYTE_ARRAY;
         StrColTask &sc = stasks[ci];
         memset(&sc, 0, sizeof(sc));
-        sc.base = dev->as<uint8_t>();
+        sc.base = dev;
         sc.data_bytes = ch.data_bytes;
         sc.rlen = (int32_t *)scratch(nrows * 4 + 16);
         sc.rsrc = (int64_t *)scratch(nrows * 8 + 16);
@@ -1177,9 +1254,9 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
                      "column chunk %d page %d: encoding %d%s", ci, p, pg.encoding,
                      pg.encoding == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : " is not supported for BYTE_ARRAY columns");
           PageTask pt;
-          pt.values = dev->as<uint8_t>() + pg.values_offset;
+          pt.values = dev + pg.values_offset;
           pt.values_bytes = pg.values_bytes;
-          pt.def = pg.def_bytes > 0 ? dev->as<uint8_t>() + pg.def_offset : nullptr;
+          pt.def = pg.def_bytes > 0 ? dev + pg.def_offset : nullptr;
           pt.def_bytes = pg.def_bytes;
           pt.row_start = row;
           pt.num_values = pg.num_values;
@@ -1210,7 +1287,7 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
       ct.dict_count = 0;
       if (ch.dict_offset >= 0 && ch.dict_count >= 0) {   // an all-NULL chunk has an empty dictionary page
         SB_REQUIRE(ch.dict_offset + (int64_t)ch.dict_count * (pw ? pw : 1) <= ch.data_bytes, "column chunk %d: dictionary overruns the chunk", ci);
-        ct.dict = dev->as<uint8_t>() + ch.dict_offset;
+        ct.dict = dev + ch.dict_offset;
         ct.dict_count = ch.dict_count;
       }
       ct.phys_width = pw;
@@ -1225,9 +1302,9 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
                    "column chunk %d page %d: encoding %d%s", ci, p, pg.encoding,
                    pg.encoding == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : " is not supported for this column");
         PageTask pt;
-        pt.values = dev->as<uint8_t>() + pg.values_offset;
+        pt.values = dev + pg.values_offset;
         pt.values_bytes = pg.values_bytes;
-        pt.def = pg.def_bytes > 0 ? dev->as<uint8_t>() + pg.def_offset : nullptr;
+        pt.def = pg.def_bytes > 0 ? dev + pg.def_offset : nullptr;
         pt.def_bytes = pg.def_bytes;
         pt.row_start = row;
         pt.num_values = pg.num_values;
@@ -1277,7 +1354,147 @@ extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_s
     if (t) table_free(t);
     throw;
   }
-  *out = t;
+  return t;
+}
+
+extern "C" int sb_scan_decode(const sb_column_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out) {
+  SB_API_BEGIN
+  require_init();
+  SB_REQUIRE(chunks && out && ncols > 0, "null argument");
+  cudaStream_t st = stream_of(s);
+  *out = scan_decode_chunks(chunks, ncols, st, [st](const sb_column_chunk &ch, std::vector<std::unique_ptr<Scratch>> &temps) {
+    // the encoded bytes cross PCIe once, as they lie in the file
+    Scratch *dev = new Scratch(ch.data_bytes + 32, st);
+    temps.emplace_back(dev);
+    if (ch.data_bytes > 0) SB_CUDA(cudaMemcpyAsync(dev->ptr, ch.data, (size_t)ch.data_bytes, cudaMemcpyHostToDevice, st));
+    return (const uint8_t *)dev->ptr;
+  });
+  SB_API_END
+}
+
+// Compressed chunks: (1) one H2D copy per chunk; (2) scan_snappy decodes every page of the call into one image per chunk (page
+// p at img_off[p], its size from the spans, so nothing is read back to allocate it); (3) scan_resolve_pages writes one record per
+// page (status, V1 level length, first bytes of the values), read back with one synchronisation; (4) the host checks them as
+// sb_parquet_chunk_pages checks the pages of a file, builds sb_page descriptors relative to the image and hands the images to
+// scan_decode_chunks.
+extern "C" int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int32_t ncols, sb_stream *s, sb_table **out) {
+  SB_API_BEGIN
+  require_init();
+  SB_REQUIRE(chunks && out && ncols > 0, "null argument");
+  cudaStream_t st = stream_of(s);
+  std::vector<std::vector<int64_t>> img_off(ncols);
+  std::vector<int64_t> img_bytes(ncols, 0);
+  std::vector<std::unique_ptr<Scratch>> raw, images;
+  std::vector<SnappyPage> sp;
+  std::vector<ResolveTask> rt_tasks;
+  std::vector<int32_t> slot_base(ncols, 0);
+  for (int ci = 0; ci < ncols; ci++) {
+    const sb_compressed_chunk &ch = chunks[ci];
+    SB_REQUIRE(ch.data && (ch.spans || ch.npages == 0) && ch.npages >= 0 && ch.data_bytes >= 0, "column chunk %d: null buffers", ci);
+    require_codec(ch.codec);
+    SB_REQUIRE(ch.max_def_level == 0 || ch.max_def_level == 1, "column chunk %d: nested schemas are not supported (max definition level %d)", ci,
+               ch.max_def_level);
+    img_off[ci].resize(ch.npages);
+    int64_t off = 0;
+    for (int p = 0; p < ch.npages; p++) {
+      const sb_page_span &x = ch.spans[p];
+      SB_REQUIRE(x.body_offset >= 0 && x.compressed_bytes >= 0 && x.uncompressed_bytes >= 0 && x.body_offset + x.compressed_bytes <= ch.data_bytes &&
+                     x.levels_bytes >= 0 && x.levels_bytes <= x.compressed_bytes && x.levels_bytes <= x.uncompressed_bytes,
+                 "column chunk %d page %d: span outside the chunk", ci, p);
+      SB_REQUIRE(x.values_compressed ? ch.codec == SB_CODEC_SNAPPY : x.compressed_bytes == x.uncompressed_bytes,
+                 "column chunk %d page %d: %s page of %d stored bytes for %d", ci, p, x.values_compressed ? "compressed" : "uncompressed",
+                 x.compressed_bytes, x.uncompressed_bytes);
+      img_off[ci][p] = off;
+      off += ((int64_t)x.uncompressed_bytes + 15) / 16 * 16;
+    }
+    img_bytes[ci] = off;
+    slot_base[ci] = (int32_t)sp.size();
+    Scratch *r = new Scratch(ch.data_bytes + 16, st), *im = new Scratch(off + 32, st);
+    raw.emplace_back(r);
+    images.emplace_back(im);
+    if (ch.data_bytes > 0) SB_CUDA(cudaMemcpyAsync(r->ptr, ch.data, (size_t)ch.data_bytes, cudaMemcpyHostToDevice, st));
+    for (int p = 0; p < ch.npages; p++) {
+      const sb_page_span &x = ch.spans[p];
+      SnappyPage t;
+      t.src = r->as<uint8_t>() + x.body_offset;
+      t.dst = im->as<uint8_t>() + img_off[ci][p];
+      t.levels_bytes = x.levels_bytes;
+      t.src_bytes = x.compressed_bytes;
+      t.dst_bytes = x.uncompressed_bytes;
+      t.compressed = x.values_compressed != 0;
+      t.slot = (int32_t)sp.size();
+      sp.push_back(t);
+      ResolveTask q;
+      q.image = t.dst;
+      q.bytes = x.uncompressed_bytes;
+      q.levels_bytes = x.page_type == 3 ? x.levels_bytes : 0;
+      q.v1_def = x.page_type == 0 && ch.max_def_level > 0;
+      q.slot = t.slot;
+      rt_tasks.push_back(q);
+    }
+  }
+  const int np = (int)sp.size();
+  std::vector<PageRecord> recs(np);
+  if (np > 0) {
+    // largest pages first: the block scheduler hands them out in order, so the longest page does not start last
+    std::vector<SnappyPage> order(sp);
+    std::stable_sort(order.begin(), order.end(), [](const SnappyPage &a, const SnappyPage &b) { return a.src_bytes > b.src_bytes; });
+    Scratch d_sp((int64_t)np * sizeof(SnappyPage), st), d_rt((int64_t)np * sizeof(ResolveTask), st), d_status((int64_t)np * 4, st),
+        d_rec((int64_t)np * sizeof(PageRecord), st);
+    SB_CUDA(cudaMemcpyAsync(d_sp.ptr, order.data(), (size_t)np * sizeof(SnappyPage), cudaMemcpyHostToDevice, st));
+    SB_CUDA(cudaMemcpyAsync(d_rt.ptr, rt_tasks.data(), (size_t)np * sizeof(ResolveTask), cudaMemcpyHostToDevice, st));
+    {
+      KernelTimer kt("scan_snappy", st);
+      launch_snappy(d_sp.as<SnappyPage>(), np, d_status.as<int32_t>(), st);
+    }
+    {
+      KernelTimer kt("scan_resolve_pages", st);
+      launch_resolve_pages(d_rt.as<ResolveTask>(), np, d_status.as<int32_t>(), d_rec.as<PageRecord>(), st);
+    }
+    SB_CUDA(cudaMemcpyAsync(recs.data(), d_rec.ptr, (size_t)np * sizeof(PageRecord), cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+  }
+  raw.clear();
+  // the page checks of sb_parquet_chunk_pages, on the decoded pages
+  std::vector<std::vector<sb_page>> pages(ncols);
+  std::vector<sb_column_chunk> dec(ncols);
+  for (int ci = 0; ci < ncols; ci++) {
+    const sb_compressed_chunk &ch = chunks[ci];
+    sb_column_chunk &d = dec[ci];
+    memset(&d, 0, sizeof(d));
+    d.type = ch.type;
+    d.scale = ch.scale;
+    d.physical_type = ch.physical_type;
+    d.data = images[ci]->as<uint8_t>();   // the image (device); scan_decode_chunks reads it through device_bytes only
+    d.data_bytes = img_bytes[ci];
+    d.dict_offset = -1;
+    for (int p = 0; p < ch.npages; p++) {
+      const sb_page_span &x = ch.spans[p];
+      const PageRecord &r = recs[slot_base[ci] + p];
+      const int64_t header_at = x.body_offset - x.header_bytes;
+      if (r.status != SNAPPY_OK)
+        fail(SB_ERR_INVALID, "column chunk %d page %d (byte %lld of the column chunk): malformed Snappy stream: %s", ci, p, (long long)header_at,
+             snappy_status_text(r.status));
+      if (x.page_type == 2) {
+        d.dict_offset = img_off[ci][p];
+        d.dict_count = x.num_values;
+        continue;
+      }
+      sb_page pg;
+      memset(&pg, 0, sizeof(pg));
+      pg.encoding = x.encoding;
+      pg.num_values = x.num_values;
+      const int dp = (int)pages[ci].size();
+      data_page_sections(pg, x.page_type == 0, ch.max_def_level, x.levels_bytes, img_off[ci][p], x.uncompressed_bytes,
+                         r.body_short ? nullptr : (const uint8_t *)&r.def_len);
+      if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED)
+        check_delta_header(r.head, std::min<int64_t>(r.head_bytes, pg.values_bytes), pg.encoding, x.num_values, dp, header_at);
+      pages[ci].push_back(pg);
+    }
+    d.pages = pages[ci].data();
+    d.npages = (int32_t)pages[ci].size();
+  }
+  *out = scan_decode_chunks(dec.data(), ncols, st, [&](const sb_column_chunk &ch, std::vector<std::unique_ptr<Scratch>> &) { return ch.data; });
   SB_API_END
 }
 

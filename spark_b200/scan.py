@@ -2,9 +2,10 @@
 
 Reference: FileSourceScanExec.doExecuteColumnar (sql/core/src/main/scala/org/apache/spark/sql/execution/DataSourceScanExec.scala:735-760)
 hands out the ColumnarBatches of VectorizedParquetRecordReader (sql/core/src/main/java/.../parquet/VectorizedParquetRecordReader.java);
-one batch here is one row group.  The footer (schema, column-chunk byte ranges) is read with pyarrow's metadata reader -- the
-role parquet-mr's ParquetFileReader plays for the reference; every data byte goes through sb_parquet_chunk_pages +
-sb_scan_decode.
+one batch here is one row group.  The footer (schema, column-chunk byte ranges, codecs) is read with pyarrow's metadata reader --
+the role parquet-mr's ParquetFileReader plays for the reference; every data byte goes through sb_parquet_chunk_pages +
+sb_scan_decode (uncompressed row groups) or sb_parquet_page_spans + sb_scan_decode_compressed (SNAPPY pages, decompressed on the
+GPU).
 """
 from __future__ import annotations
 
@@ -70,6 +71,36 @@ class EncodedColumnChunk:
         return EncodedColumnChunk(sb_type, scale, physical, buf, pages, npages.value, doff.value, dcount.value)
 
 
+class CompressedColumnChunk:
+    """Host bytes of one column chunk as it lies in the file + the spans of its pages (sb_parquet_page_spans)."""
+
+    def __init__(self, sb_type, scale, physical, codec, max_def_level, data: np.ndarray, spans, npages):
+        self.type, self.scale, self.physical, self.codec, self.max_def_level = sb_type, scale, physical, codec, max_def_level
+        self.data, self.spans, self.npages = data, spans, npages
+
+    @property
+    def nbytes(self):
+        return int(self.data.nbytes)
+
+    def c(self) -> capi.sb_compressed_chunk:
+        s = capi.sb_compressed_chunk()
+        s.type, s.scale, s.physical_type, s.codec = self.type, self.scale, self.physical, self.codec
+        s.max_def_level, s.npages = self.max_def_level, self.npages
+        s.data = self.data.ctypes.data
+        s.data_bytes = self.data.nbytes
+        s.spans = C.cast(self.spans, C.POINTER(capi.sb_page_span))
+        return s
+
+    @staticmethod
+    def from_file_bytes(buf: np.ndarray, sb_type, scale, physical, codec, max_def_level, cap=None) -> "CompressedColumnChunk":
+        lib = capi.load()
+        cap = cap or max(16, buf.nbytes // 64 + 16)          # a page header alone takes more than 16 bytes
+        spans = (capi.sb_page_span * cap)()
+        n = C.c_int32()
+        capi.check(lib.sb_parquet_page_spans(buf.ctypes.data, buf.nbytes, codec, max_def_level, spans, cap, C.byref(n)))
+        return CompressedColumnChunk(sb_type, scale, physical, codec, max_def_level, buf, spans, n.value)
+
+
 def decode_chunks(names, chunks, stream=None, arrow_types=None) -> ColumnarBatch:
     lib = capi.load()
     arr = (capi.sb_column_chunk * len(chunks))()
@@ -80,9 +111,21 @@ def decode_chunks(names, chunks, stream=None, arrow_types=None) -> ColumnarBatch
     return ColumnarBatch(h, list(names), arrow_types)
 
 
+def decode_file_chunks(names, chunks, stream=None, arrow_types=None) -> ColumnarBatch:
+    """sb_scan_decode_compressed of CompressedColumnChunks (each chunk's codec is its own)"""
+    lib = capi.load()
+    arr = (capi.sb_compressed_chunk * len(chunks))()
+    for i, ch in enumerate(chunks):
+        arr[i] = ch.c()
+    h = C.c_void_p()
+    capi.check(lib.sb_scan_decode_compressed(arr, len(chunks), _h(stream), C.byref(h)))
+    return ColumnarBatch(h, list(names), arrow_types)
+
+
 class ParquetScanExec(SparkPlan):
     """Scan of a Parquet file: `batches()` yields one HBM-resident ColumnarBatch per row group; executeColumnar concatenates
-    them (for plans that want the partition as one batch).  Pages must be uncompressed."""
+    them (for plans that want the partition as one batch).  Pages may be uncompressed or SNAPPY-compressed (per column);
+    other codecs and nested columns are refused with SparkB200Error(5)."""
 
     def __init__(self, path, columns=None):
         self.path = path
@@ -95,29 +138,57 @@ class ParquetScanExec(SparkPlan):
         self._mm = mmap.mmap(self._f.fileno(), 0, access=mmap.ACCESS_READ)
         self._bytes = np.frombuffer(self._mm, dtype=np.uint8)
 
-    def row_group_chunks(self, rg: int):
+    def _column_metas(self, rg: int):
+        """(field, column-chunk metadata) of every selected column of row group rg; nested columns are refused"""
         g = self.meta.row_group(rg)
         by_name = {g.column(i).path_in_schema: g.column(i) for i in range(g.num_columns)}
         out = []
         for f in self.fields:
+            if f.name not in by_name:
+                raise capi.SparkB200Error(5, "column %s is nested (%s); the GPU scan reads flat columns" % (f.name, f.type))
             cm = by_name[f.name]
-            if cm.compression != "UNCOMPRESSED":
-                raise capi.SparkB200Error(5, "column %s is %s-compressed; the GPU scan reads uncompressed pages" % (f.name, cm.compression))
             if cm.physical_type not in _PHYS:
                 raise capi.SparkB200Error(5, "column %s: physical type %s is not supported by the GPU scan" % (f.name, cm.physical_type))
             if (cm.physical_type == "BYTE_ARRAY") != _is_bytes(f.type):
                 raise capi.SparkB200Error(5, "column %s: physical type %s with Arrow type %s is not supported by the GPU scan" % (f.name, cm.physical_type, f.type))
-            start = cm.dictionary_page_offset if cm.has_dictionary_page and cm.dictionary_page_offset else cm.data_page_offset
-            start = min(start, cm.data_page_offset)
-            buf = self._bytes[start:start + cm.total_compressed_size]
-            t, scale = _sb_type(f.type)
-            max_def = self.file.schema.column(self.file.schema.names.index(f.name)).max_definition_level
+            out.append((f, cm))
+        return out
+
+    def _chunk_bytes(self, f, cm):
+        start = cm.dictionary_page_offset if cm.has_dictionary_page and cm.dictionary_page_offset else cm.data_page_offset
+        start = min(start, cm.data_page_offset)
+        t, scale = _sb_type(f.type)
+        max_def = self.file.schema.column(self.file.schema.names.index(f.name)).max_definition_level
+        return self._bytes[start:start + cm.total_compressed_size], t, scale, max_def
+
+    def row_group_chunks(self, rg: int):
+        """host page descriptors of the row group's chunks, which must be uncompressed"""
+        out = []
+        for f, cm in self._column_metas(rg):
+            if cm.compression != "UNCOMPRESSED":
+                raise capi.SparkB200Error(5, "column %s is %s-compressed; the GPU scan reads uncompressed pages" % (f.name, cm.compression))
+            buf, t, scale, max_def = self._chunk_bytes(f, cm)
             out.append(EncodedColumnChunk.from_file_bytes(buf, t, scale, _PHYS[cm.physical_type], max_def))
         return out
 
+    def row_group_file_chunks(self, rg: int):
+        """the row group's chunks as they lie in the file, with the spans of their pages (UNCOMPRESSED or SNAPPY)"""
+        out = []
+        for f, cm in self._column_metas(rg):
+            codec = capi.SB_CODEC.get(cm.compression)
+            if codec not in (capi.SB_CODEC["UNCOMPRESSED"], capi.SB_CODEC["SNAPPY"]):
+                raise capi.SparkB200Error(5, "column %s is %s-compressed; the GPU scan reads UNCOMPRESSED and SNAPPY pages" % (f.name, cm.compression))
+            buf, t, scale, max_def = self._chunk_bytes(f, cm)
+            out.append(CompressedColumnChunk.from_file_bytes(buf, t, scale, _PHYS[cm.physical_type], codec, max_def))
+        return out
+
     def batches(self, stream=None):
+        types = [f.type for f in self.fields]
         for rg in range(self.meta.num_row_groups):
-            yield decode_chunks(self.columns, self.row_group_chunks(rg), stream, [f.type for f in self.fields])
+            if all(cm.compression == "UNCOMPRESSED" for _, cm in self._column_metas(rg)):
+                yield decode_chunks(self.columns, self.row_group_chunks(rg), stream, types)          # no synchronisation
+            else:
+                yield decode_file_chunks(self.columns, self.row_group_file_chunks(rg), stream, types)
 
     def executeColumnar(self, stream=None):
         bs = list(self.batches(stream))
