@@ -303,6 +303,24 @@ int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *dictionary, i
 #define SB_OP_STR_LIKE 59          /* slice = the pattern (UTF-8); arg2 = the escape character (a code point <= 0xFFFF, usually '\\').
                                       `_` matches one code point, `%` any run of them, newlines included */
 #define SB_OP_STR_OCTET_LENGTH 60  /* I32: the byte length; the slice is empty */
+#define SB_OP_STR_CHAR_LENGTH 61   /* I32: the code points (Length, UTF8String.numChars: one per lead byte, stepping by the width the
+                                      lead byte declares, so ill-formed bytes count as Spark counts them); the slice is empty */
+
+/* string-producing programs (sb_string_project, csrc/strfunc.cu): postfix lists of the nodes below, vtype 0, whose value is a
+ * string.  Literal slices are lit.i = offset << 32 | length of sb_expr.bytes, as for the string tests.  Semantics are
+ * UTF8String's (UTF8_BINARY, non-ANSI); code points are stepped by the width each lead byte declares.  A value is assembled from
+ * at most SB_SF_MAX_RANGES byte ranges (a pad counts as one), which validation checks statically. */
+#define SB_OP_SF_COL 70            /* push string column `arg` */
+#define SB_OP_SF_LIT 71            /* push the literal slice; arg2 = 1: a NULL string */
+#define SB_OP_SF_SUBSTRING 72      /* pop s; push substringSQL(s, pos = arg, len = arg2) */
+#define SB_OP_SF_CONCAT 73         /* pop `arg` >= 1 strings; push their concatenation, NULL if any is NULL */
+#define SB_OP_SF_CONCAT_WS 74      /* pop `arg` >= 1 strings; push them joined by the literal separator, NULL ones skipped */
+#define SB_OP_SF_TRIM 75           /* pop s; arg = 0: trim() (ASCII spaces); arg = 1: trim(trimStr), trimStr = the literal */
+#define SB_OP_SF_LTRIM 76
+#define SB_OP_SF_RTRIM 77
+#define SB_OP_SF_LPAD 78           /* pop s; push lpad(s, len = arg, pad = the literal) */
+#define SB_OP_SF_RPAD 79
+#define SB_SF_MAX_RANGES 16
 
 /* value class of a node's result */
 #define SB_VT_BOOL 1
@@ -330,6 +348,10 @@ typedef struct sb_expr {
  * predicate may be NULL (no filter); each projection becomes one output column. */
 int sb_filter_project(const sb_table *in, const sb_expr *predicate, const sb_expr *projections, int32_t nproj,
                       sb_stream *s, sb_table **out);
+/* ProjectExec of string-producing functions: one SB_STRING column per program (SB_OP_SF_* nodes, out_type SB_STRING).  Every
+ * program is validated before anything is launched.  The call synchronises the stream once, to read back the arena sizes; an
+ * arena above 2^31 - 1 bytes is SB_ERR_UNSUPPORTED naming the output. */
+int sb_string_project(const sb_table *in, const sb_expr *programs, int32_t nprog, sb_stream *s, sb_table **out);
 
 /* ---- ShuffleExchangeExec, map side (SQLX/exchange/ShuffleExchangeExec.scala:359-619) ---------
  * partition id = pmod(Murmur3Hash(keys, 42), n): bit-exact with HashPartitioning.partitionIdExpression

@@ -33,6 +33,7 @@ public final class Native {
   public static native void tableRetain(long table);
   public static native void tableRelease(long table);
   public static native long tableSelect(long table, int[] columns);
+  public static native long tableZip(long a, long b);           // the columns of a then b; equal row counts, shares buffers
   public static native long tableSlice(long table, long begin, long end, long stream);
   public static native long tableConcat(long[] tables, long stream);
 
@@ -48,6 +49,8 @@ public final class Native {
   public static native long exprCreate(int[] ops, int[] vtypes, int[] args, int[] args2, long[] literals, byte[] bytes, int outType);
   public static native void exprFree(long expr);
   public static native long filterProject(long table, long predicateExpr, long[] projectionExprs, long stream);
+  /** string-producing programs (exprCreate with SB_OP_SF_* nodes, outType STRING): one string column each (sb_string_project). */
+  public static native long stringProject(long table, long[] programExprs, long stream);
 
   // ---- ShuffleExchangeExec ------------------------------------------------------------------------------------------------
   /** returns the partitioned table; offsetsOut receives numPartitions + 1 boundaries. */

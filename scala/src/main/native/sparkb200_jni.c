@@ -202,6 +202,19 @@ NATIVE(jlong, filterProject)(JNIEnv *env, jclass c, jlong table, jlong predicate
   return (jlong)(intptr_t)out;
 }
 
+NATIVE(jlong, stringProject)(JNIEnv *env, jclass c, jlong table, jlongArray programExprs, jlong stream) {
+  jsize np = (*env)->GetArrayLength(env, programExprs);
+  jlong *p = (*env)->GetLongArrayElements(env, programExprs, NULL);
+  sb_expr *progs = (sb_expr *)calloc((size_t)(np ? np : 1), sizeof(sb_expr));
+  for (jsize i = 0; i < np; i++) progs[i] = *(const sb_expr *)(intptr_t)p[i];
+  sb_table *out = NULL;
+  int rc = sb_string_project(TBL(table), progs, np, STR(stream), &out);
+  free(progs);
+  (*env)->ReleaseLongArrayElements(env, programExprs, p, JNI_ABORT);
+  throw_if(env, rc);
+  return (jlong)(intptr_t)out;
+}
+
 NATIVE(jlong, roundRobinPartition)(JNIEnv *env, jclass c, jlong table, jint start, jint n, jlong stream, jlongArray offsetsOut) {
   jlong *offs = (*env)->GetLongArrayElements(env, offsetsOut, NULL);
   sb_table *out = NULL;
@@ -296,6 +309,11 @@ NATIVE(jlong, tableSelect)(JNIEnv *env, jclass c, jlong table, jintArray columns
   int rc = sb_table_select(TBL(table), (const int32_t *)k, n, &out);
   (*env)->ReleaseIntArrayElements(env, columns, k, JNI_ABORT);
   throw_if(env, rc);
+  return (jlong)(intptr_t)out;
+}
+NATIVE(jlong, tableZip)(JNIEnv *env, jclass c, jlong a, jlong b) {
+  sb_table *out = NULL;
+  throw_if(env, sb_table_zip(TBL(a), TBL(b), &out));
   return (jlong)(intptr_t)out;
 }
 NATIVE(jlong, tableSlice)(JNIEnv *env, jclass c, jlong table, jlong begin, jlong end, jlong stream) {

@@ -69,7 +69,8 @@ case class GpuHashAggregateExec(
   override protected def withNewChildInternal(c: SparkPlan): SparkPlan = copy(child = c)
 }
 
-/** FilterExec / ProjectExec (basicPhysicalOperators.scala:245 / :47) as one pass per batch: sb_filter_project. */
+/** FilterExec / ProjectExec (basicPhysicalOperators.scala:245 / :47) as one pass per batch: sb_filter_project; with string-producing
+ *  functions, sb_string_project too (GpuSupport.runStringStage). */
 case class GpuFilterProjectExec(condition: Option[Expression], projectList: Seq[NamedExpression], child: SparkPlan)
   extends UnaryExecNode with GpuExec {
   override def output: Seq[Attribute] = projectList.map(_.toAttribute)
@@ -77,15 +78,29 @@ case class GpuFilterProjectExec(condition: Option[Expression], projectList: Seq[
   override protected def doExecuteColumnar(): RDD[ColumnarBatch] = {
     val childTypes = child.output.map(_.dataType).toArray
     val outTypes = output.map(_.dataType).toArray
-    val compiled = GpuSupport.compileFilterProject(condition, projectList, child.output)
-    child.executeColumnar().mapPartitions { batches =>
-      val stream = taskStream()
-      val native = compiled.lower()
-      Option(org.apache.spark.TaskContext.get()).foreach(_.addTaskCompletionListener[Unit](_ => native.close()))
-      batches.map { b =>
-        val in = DeviceTransfer.toDevice(b, childTypes, stream)
-        try new DeviceBatch(Native.filterProject(in.table, native.filterExpr, native.inputExprs, stream), outTypes): ColumnarBatch
-        finally in.close()
+    if (GpuSupport.hasStringFunction(condition, projectList)) {
+      val stage = GpuSupport.compileStringStage(condition, projectList, child.output)
+      child.executeColumnar().mapPartitions { batches =>
+        val stream = taskStream()
+        val native = stage.lower()
+        Option(org.apache.spark.TaskContext.get()).foreach(_.addTaskCompletionListener[Unit](_ => native.close()))
+        batches.map { b =>
+          val in = DeviceTransfer.toDevice(b, childTypes, stream)
+          try new DeviceBatch(GpuSupport.runStringStage(native, in.table, stream), outTypes): ColumnarBatch
+          finally in.close()
+        }
+      }
+    } else {
+      val compiled = GpuSupport.compileFilterProject(condition, projectList, child.output)
+      child.executeColumnar().mapPartitions { batches =>
+        val stream = taskStream()
+        val native = compiled.lower()
+        Option(org.apache.spark.TaskContext.get()).foreach(_.addTaskCompletionListener[Unit](_ => native.close()))
+        batches.map { b =>
+          val in = DeviceTransfer.toDevice(b, childTypes, stream)
+          try new DeviceBatch(Native.filterProject(in.table, native.filterExpr, native.inputExprs, stream), outTypes): ColumnarBatch
+          finally in.close()
+        }
       }
     }
   }

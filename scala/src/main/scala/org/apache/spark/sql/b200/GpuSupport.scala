@@ -77,7 +77,13 @@ object GpuSupport {
       case _ => false
     })
   def supports(b: BroadcastExchangeExec): Boolean = outputOk(b.child) && !b.child.output.exists(_.dataType == StringType)
-  def supports(f: FilterExec): Boolean = outputOk(f.child) && exprOk(f.condition)
+  def supports(f: FilterExec): Boolean = outputOk(f.child) && hoistedOk(f.condition)
+  /** an expression of a numeric / boolean program once every string-producing function inside it is a hidden column of its own
+   *  (csrc/strfunc.cu): the condition of a FilterExec, a numeric output of a ProjectExec */
+  private def hoistedOk(e: Expression): Boolean = {
+    val hidden = new ArrayBuffer[(AttributeReference, Expression)]()
+    exprOk(ExprCompiler.hoist(e, hidden)) && hidden.forall(h => ExprCompiler.stringProgramOk(h._2))
+  }
   def supports(e: ExpandExec): Boolean = outputOk(e.child) && e.output.forall(a => fixedWidth(a.dataType) || a.dataType == StringType) &&
     e.projections.forall(_.forall(exprOk))
   def supports(w: WindowExec): Boolean = outputOk(w.child) && lowerWindow(w).isDefined
@@ -137,7 +143,9 @@ object GpuSupport {
     Some(WindowLowered(ordinals(w.partitionSpec, in), oc, asc, nf, f.map(_._1).toArray, f.map(_._2).toArray, f.map(_._3).toArray,
       f.map(_._4).toArray, f.map(_._5).toArray, f.map(_._6).toArray))
   }
-  def supports(p: ProjectExec): Boolean = outputOk(p.child) && p.projectList.forall(e => exprOk(e) && typeOk(e.dataType))
+  def supports(p: ProjectExec): Boolean = outputOk(p.child) && p.projectList.forall(e =>
+    typeOk(e.dataType) && (ExprCompiler.stringProgramOk(stripAlias(e)) || hoistedOk(e)))
+  private def stripAlias(e: Expression): Expression = e match { case Alias(c, _) => stripAlias(c); case o => o }
 
   private def keyBits(dt: DataType): Int = dt match {
     case BooleanType | ByteType => 8
@@ -207,6 +215,71 @@ object GpuSupport {
   def compileFilterProject(condition: Option[Expression], projectList: Seq[NamedExpression], in: Seq[Attribute]): Lowerable =
     Lowerable(Array.empty, Array.empty, projectList.map(p => Option(ExprCompiler.compile(p, in))).toArray,
       condition.map(ExprCompiler.compile(_, in)))
+
+  // ---- FilterExec / ProjectExec with string-producing functions: Native.stringProject for string-valued outputs and for the string
+  // functions inside the condition and the numeric outputs (hidden columns), Native.filterProject for the rest, Native.tableZip to
+  // join them and Native.tableSelect for the projection's order.  The condition runs first, so the projections see surviving rows only.
+  def hasStringFunction(condition: Option[Expression], projectList: Seq[NamedExpression]): Boolean =
+    (condition.toSeq ++ projectList).exists(_.find(ExprCompiler.stringFunction).isDefined)
+
+  final class StringStageHandles(val condHidden: Array[Long], val cond: Long, val keep: Array[Long], val strings: Array[Long],
+                                 val projHidden: Array[Long], val numeric: Array[Long], val order: Array[Int]) {
+    def close(): Unit = (condHidden ++ keep ++ strings ++ projHidden ++ numeric :+ cond).foreach(h => if (h != 0L) Native.exprFree(h))
+  }
+  final case class StringStage(condHidden: Array[ExprCompiler.Program], cond: Option[ExprCompiler.Program], keep: Array[ExprCompiler.Program],
+                               strings: Array[ExprCompiler.Program], projHidden: Array[ExprCompiler.Program],
+                               numeric: Array[ExprCompiler.Program], order: Array[Int]) {
+    def lower(): StringStageHandles = new StringStageHandles(condHidden.map(_.create()), cond.map(_.create()).getOrElse(0L),
+      keep.map(_.create()), strings.map(_.create()), projHidden.map(_.create()), numeric.map(_.create()), order)
+  }
+
+  def compileStringStage(condition: Option[Expression], projectList: Seq[NamedExpression], in: Seq[Attribute]): StringStage = {
+    val ch = new ArrayBuffer[(AttributeReference, Expression)]()
+    val cond = condition.map(ExprCompiler.hoist(_, ch))
+    val condIn = in ++ ch.map(_._1)
+    val isString = projectList.map(p => ExprCompiler.stringFunction(stripAlias(p)))
+    val ph = new ArrayBuffer[(AttributeReference, Expression)]()
+    val numericExprs = projectList.zip(isString).collect { case (p, false) => ExprCompiler.hoist(p, ph) }
+    val projIn = in ++ ph.map(_._1)
+    var ni = -1
+    var si = numericExprs.length - 1
+    val order = isString.map(str => if (str) { si += 1; si } else { ni += 1; ni }).toArray   // numeric outputs first, then the strings
+    StringStage(ch.map(h => ExprCompiler.compileString(h._2, in)).toArray, cond.map(ExprCompiler.compile(_, condIn)),
+      in.map(a => ExprCompiler.compile(a, condIn)).toArray,
+      projectList.zip(isString).collect { case (p, true) => ExprCompiler.compileString(p, in) }.toArray,
+      ph.map(h => ExprCompiler.compileString(h._2, in)).toArray, numericExprs.map(ExprCompiler.compile(_, projIn)).toArray, order)
+  }
+
+  /** one batch through a lowered StringStage; returns a new table */
+  def runStringStage(h: StringStageHandles, table: Long, stream: Long): Long = {
+    def withHidden(t: Long, progs: Array[Long]): Long =            // t ++ the string columns of progs (a new reference)
+      if (progs.isEmpty) { Native.tableRetain(t); t }
+      else { val s = Native.stringProject(t, progs, stream); try Native.tableZip(t, s) finally Native.tableRelease(s) }
+    Native.tableRetain(table)
+    var cur = table
+    try {
+      if (h.cond != 0L) {
+        val w = withHidden(cur, h.condHidden)
+        val kept = try Native.filterProject(w, h.cond, h.keep, stream) finally Native.tableRelease(w)
+        Native.tableRelease(cur)
+        cur = kept
+      }
+      val parts = new ArrayBuffer[Long]()
+      try {
+        if (h.numeric.nonEmpty) {
+          val w = withHidden(cur, h.projHidden)
+          parts += (try Native.filterProject(w, 0L, h.numeric, stream) finally Native.tableRelease(w))
+        }
+        if (h.strings.nonEmpty) parts += Native.stringProject(cur, h.strings, stream)
+        if (parts.isEmpty) Native.tableSelect(cur, Array.empty[Int])
+        else if (parts.length == 1) Native.tableSelect(parts(0), h.order)
+        else {
+          val all = Native.tableZip(parts(0), parts(1))
+          try Native.tableSelect(all, h.order) finally Native.tableRelease(all)
+        }
+      } finally parts.foreach(Native.tableRelease)
+    } finally Native.tableRelease(cur)
+  }
 
   def ordinals(keys: Seq[Expression], in: Seq[Attribute]): Array[Int] =
     keys.map { case a: AttributeReference => in.indexWhere(_.exprId == a.exprId) }.toArray
@@ -354,6 +427,7 @@ object ExprCompiler {
     case Contains(c, l) => strCol(c) && strLit(l)
     case Like(c, l, _) => strCol(c) && strLit(l)
     case OctetLength(c) => strCol(c)
+    case Length(c) => strCol(c)
     case a: AttributeReference => GpuExec.typeId(a.dataType) > 0
     case Alias(c, _) => supported(c)
     case l: Literal => vt(l.dataType) > 0        // a NULL literal too: LIT_NULL carries its class (an untyped NULL has none)
@@ -371,6 +445,88 @@ object ExprCompiler {
     case Cast(c, to, _, _) => vt(to) > 1 && vt(c.dataType) > 0 && supported(c)
     case _ => false
   }
+  // ---- string-producing functions (csrc/strfunc.cu, SB_OP_SF_*): programs of their own, run by Native.stringProject.  Positions,
+  // lengths and pad lengths are int literals; trim strings, pads and separators string literals (NULL gives the function's NULL);
+  // string operands are UTF8_BINARY columns, string literals or other such functions.
+  private def intLit(e: Expression): Boolean = e match { case Literal(_, IntegerType) => true; case _ => false }
+  private def strArg(e: Expression): Boolean = e match { case Literal(_, dt) => binaryString(dt); case _ => false }
+  private def strOperand(e: Expression): Boolean = e match {
+    case a: AttributeReference => binaryString(a.dataType)
+    case Literal(_, dt) => binaryString(dt)
+    case _ => stringFunction(e)
+  }
+  def stringFunction(e: Expression): Boolean = binaryString(e.dataType) && (e match {
+    case Substring(s, p, l) => strOperand(s) && intLit(p) && intLit(l)
+    case Concat(cs) => cs.forall(strOperand)
+    case ConcatWs(sep +: cs) => strArg(sep) && cs.forall(strOperand)
+    case StringTrim(s, t) => strOperand(s) && t.forall(strArg)
+    case StringTrimLeft(s, t) => strOperand(s) && t.forall(strArg)
+    case StringTrimRight(s, t) => strOperand(s) && t.forall(strArg)
+    case StringLPad(s, l, p) => strOperand(s) && intLit(l) && strArg(p)
+    case StringRPad(s, l, p) => strOperand(s) && intLit(l) && strArg(p)
+    case _ => false
+  })
+  /** byte ranges a value is assembled from (SB_SF_MAX_RANGES = 16); a node never has fewer than its operands together */
+  private def ranges(e: Expression): Int = e match {
+    case Concat(cs) => math.max(1, cs.map(ranges).sum)
+    case ConcatWs(_ +: cs) => math.max(1, cs.map(ranges).sum + cs.length - 1)
+    case StringLPad(s, _, _) => ranges(s) + 1
+    case StringRPad(s, _, _) => ranges(s) + 1
+    case Substring(s, _, _) => ranges(s)
+    case StringTrim(s, _) => ranges(s)
+    case StringTrimLeft(s, _) => ranges(s)
+    case StringTrimRight(s, _) => ranges(s)
+    case _ => 1
+  }
+  def stringProgramOk(e: Expression): Boolean = stringFunction(e) && ranges(e) <= 16
+  /** `e` with every string function replaced by a hidden string column; the (column, function) pairs are appended to `out` */
+  def hoist(e: Expression, out: ArrayBuffer[(AttributeReference, Expression)]): Expression = e.transformDown {
+    case f if stringFunction(f) =>
+      val a = AttributeReference(s"_sf${out.length}", f.dataType, f.nullable)()
+      out += ((a, f))
+      a
+  }
+  def compileString(e: Expression, in: Seq[Attribute]): Program = {
+    val ops = new ArrayBuffer[Int](); val args = new ArrayBuffer[Int](); val args2 = new ArrayBuffer[Int](); val lits = new ArrayBuffer[Long]()
+    val pool = new java.io.ByteArrayOutputStream()
+    def emit(op: Int, arg: Int = 0, lit: Long = 0L, arg2: Int = 0): Unit = { ops += op; args += arg; lits += lit; args2 += arg2 }
+    def slice(b: Array[Byte]): Long = { val off = pool.size().toLong; pool.write(b, 0, b.length); (off << 32) | b.length.toLong }
+    def intOf(l: Expression): Option[Int] = Option(l.asInstanceOf[Literal].value).map(_.asInstanceOf[Int])
+    def strOf(l: Expression): Option[Array[Byte]] = Option(l.asInstanceOf[Literal].value).map(_.asInstanceOf[UTF8String].getBytes)
+    def nullString(): Unit = emit(71, 0, 0L, 1)                          // SB_OP_SF_LIT, arg2 = 1: NULL
+    def trim(op: Int, s: Expression, t: Option[Expression]): Unit = t match {
+      case None => go(s); emit(op)
+      case Some(l) => strOf(l) match { case Some(b) => go(s); emit(op, 1, slice(b)); case None => nullString() }
+    }
+    def pad(op: Int, s: Expression, l: Expression, p: Expression): Unit = (intOf(l), strOf(p)) match {
+      case (Some(n), Some(b)) => go(s); emit(op, n, slice(b))
+      case _ => nullString()
+    }
+    def go(x: Expression): Unit = x match {
+      case Alias(c, _) => go(c)
+      case a: AttributeReference => emit(70, in.indexWhere(_.exprId == a.exprId))
+      case Literal(null, _) => nullString()
+      case Literal(v, _) => emit(71, 0, slice(v.asInstanceOf[UTF8String].getBytes))
+      case Substring(s, p, l) => (intOf(p), intOf(l)) match {
+        case (Some(pi), Some(li)) => go(s); emit(72, pi, 0L, li)
+        case _ => nullString()
+      }
+      case Concat(cs) => if (cs.isEmpty) emit(71, 0, slice(Array.emptyByteArray)) else { cs.foreach(go); emit(73, cs.length) }
+      case ConcatWs(sep +: cs) => strOf(sep) match {
+        case None => nullString()
+        case Some(b) => if (cs.isEmpty) emit(71, 0, slice(Array.emptyByteArray)) else { cs.foreach(go); emit(74, cs.length, slice(b)) }
+      }
+      case StringTrim(s, t) => trim(75, s, t)
+      case StringTrimLeft(s, t) => trim(76, s, t)
+      case StringTrimRight(s, t) => trim(77, s, t)
+      case StringLPad(s, l, p) => pad(78, s, l, p)
+      case StringRPad(s, l, p) => pad(79, s, l, p)
+      case other => throw new B200Exception(5, s"string function $other is not supported on the GPU path")
+    }
+    go(e)
+    Program(ops.toArray, Array.fill(ops.length)(0), args.toArray, args2.toArray, lits.toArray, pool.toByteArray, GpuExec.typeId(StringType))
+  }
+
   def compile(e: Expression, in: Seq[Attribute]): Program = {
     val ops = new ArrayBuffer[Int](); val vts = new ArrayBuffer[Int](); val args = new ArrayBuffer[Int](); val lits = new ArrayBuffer[Long]()
     val args2 = new ArrayBuffer[Int](); val pool = new java.io.ByteArrayOutputStream()
@@ -400,6 +556,7 @@ object ExprCompiler {
       case Contains(c, l) => strTest(58, c, l)
       case Like(c, l, esc) => strTest(59, c, l, esc.toInt)
       case OctetLength(c) => emit(60, 2, colOf(c))
+      case Length(c) => emit(61, 2, colOf(c))        // SB_OP_STR_CHAR_LENGTH: code points as UTF8String.numChars counts them
       case a: AttributeReference => emit(1, vt(a.dataType), in.indexWhere(_.exprId == a.exprId))
       case Alias(c, _) => go(c)
       case Literal(null, dt) => emit(4, vt(dt))

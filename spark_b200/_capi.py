@@ -20,7 +20,10 @@ SB_OK = 0
 SB_OP = dict(COL=1, LIT_I64=2, LIT_F64=3, LIT_NULL=4, ADD=10, SUB=11, MUL=12, DIV=13, NEG=14, EQ=20, NE=21, LT=22,
              LE=23, GT=24, GE=25, AND=30, OR=31, NOT=32, ISNULL=33, ISNOTNULL=34, CAST_F64=40, CAST_I64=41, CAST_I32=42,
              STR_EQ=50, STR_LT=51, STR_LE=52, STR_GT=53, STR_GE=54, STR_IN=55, STR_STARTS_WITH=56, STR_ENDS_WITH=57, STR_CONTAINS=58,
-             STR_LIKE=59, STR_OCTET_LENGTH=60)
+             STR_LIKE=59, STR_OCTET_LENGTH=60, STR_CHAR_LENGTH=61,
+             SF_COL=70, SF_LIT=71, SF_SUBSTRING=72, SF_CONCAT=73, SF_CONCAT_WS=74, SF_TRIM=75, SF_LTRIM=76, SF_RTRIM=77, SF_LPAD=78,
+             SF_RPAD=79)
+SB_SF_MAX_RANGES = 16
 SB_VT_BOOL, SB_VT_I32, SB_VT_I64, SB_VT_F64 = 1, 2, 3, 4
 SB_AGG = dict(sum=1, avg=2, count=3, count_star=4, min=5, max=6)
 SB_AGG_MODE = dict(partial=1, final=2, complete=3, partial_merge=4)
@@ -150,6 +153,7 @@ _SIGNATURES = {
     "sb_scan_decode_compressed": [C.POINTER(sb_compressed_chunk), _i32, _p, _pp],
     "sb_scan_encode": [_p, _i32, _p, _i64, _p, _pp, C.POINTER(sb_page), _i32, C.POINTER(_i32), C.POINTER(_i64), C.POINTER(_i32)],
     "sb_filter_project": [_p, C.POINTER(sb_expr), C.POINTER(sb_expr), _i32, _p, _pp],
+    "sb_string_project": [_p, C.POINTER(sb_expr), _i32, _p, _pp],
     "sb_partition_ids": [_p, C.POINTER(_i32), _i32, _i32, _p, _p],
     "sb_hash_partition": [_p, C.POINTER(_i32), _i32, _i32, _p, _pp, C.POINTER(_i64)],
     "sb_round_robin_partition": [_p, _i32, _i32, _p, _pp, C.POINTER(_i64)],

@@ -328,7 +328,7 @@ static int build_tree(const sb_expr &e, std::vector<ExprTree> &t) {
     switch (nd.op) {
       case SB_OP_COL: case SB_OP_LIT_I64: case SB_OP_LIT_F64: case SB_OP_LIT_NULL: break;
       case SB_OP_STR_EQ: case SB_OP_STR_LT: case SB_OP_STR_LE: case SB_OP_STR_GT: case SB_OP_STR_GE: case SB_OP_STR_IN:
-      case SB_OP_STR_STARTS_WITH: case SB_OP_STR_ENDS_WITH: case SB_OP_STR_CONTAINS: case SB_OP_STR_LIKE: case SB_OP_STR_OCTET_LENGTH: break;
+      case SB_OP_STR_STARTS_WITH: case SB_OP_STR_ENDS_WITH: case SB_OP_STR_CONTAINS: case SB_OP_STR_LIKE: case SB_OP_STR_OCTET_LENGTH: case SB_OP_STR_CHAR_LENGTH: break;
       case SB_OP_NEG: case SB_OP_NOT: case SB_OP_ISNULL: case SB_OP_ISNOTNULL:
       case SB_OP_CAST_F64: case SB_OP_CAST_I64: case SB_OP_CAST_I32:
         nd.l = stack.back(); stack.pop_back(); break;

@@ -315,7 +315,7 @@ __device__ __forceinline__ void eval_row(const DevProg &p, int64_t row, int64_t 
         } else st[sp - 1] = (int64_t)(int32_t)(uint32_t)st[sp - 1];
         break;
       case SB_OP_STR_EQ: case SB_OP_STR_LT: case SB_OP_STR_LE: case SB_OP_STR_GT: case SB_OP_STR_GE: case SB_OP_STR_IN:
-      case SB_OP_STR_STARTS_WITH: case SB_OP_STR_ENDS_WITH: case SB_OP_STR_CONTAINS: case SB_OP_STR_LIKE: case SB_OP_STR_OCTET_LENGTH: {
+      case SB_OP_STR_STARTS_WITH: case SB_OP_STR_ENDS_WITH: case SB_OP_STR_CONTAINS: case SB_OP_STR_LIKE: case SB_OP_STR_OCTET_LENGTH: case SB_OP_STR_CHAR_LENGTH: {
         const int c = nd.arg;
         const bool v = bit_valid(p.col_valid[c], row);
         int64_t x = 0;

@@ -102,7 +102,7 @@ int32_t strpred_validate(const sb_table *in, const sb_expr &e, int i) {
   const sb_expr_node &nd = e.nodes[i];
   SB_REQUIRE(nd.arg >= 0 && nd.arg < (int)in->cols.size(), "string test node %d references column %d of %zu", i, nd.arg, in->cols.size());
   SB_REQUIRE(in->cols[nd.arg].type == SB_STRING, "string test node %d: column %d has type %d, not STRING", i, nd.arg, in->cols[nd.arg].type);
-  const int32_t want = nd.op == SB_OP_STR_OCTET_LENGTH ? SB_VT_I32 : SB_VT_BOOL;
+  const int32_t want = strpred_is_length(nd.op) ? SB_VT_I32 : SB_VT_BOOL;
   SB_REQUIRE(nd.vtype == want, "string test node %d (op %d): vtype %d, expected %d", i, nd.op, nd.vtype, want);
   const uint64_t off = (uint64_t)nd.lit.i >> 32, len = (uint64_t)nd.lit.i & 0xffffffffu;
   SB_REQUIRE(e.nbytes >= 0 && off + len <= (uint64_t)e.nbytes && (len == 0 || e.bytes), "string test node %d: literal [%llu, +%llu) lies outside the %lld pool bytes",
@@ -117,8 +117,8 @@ int32_t strpred_validate(const sb_table *in, const sb_expr &e, int i) {
       SB_REQUIRE(nd.arg2 >= 1 && nd.arg2 <= 0xFFFF, "STR_LIKE node %d: escape character %d is not a code point in 1..0xFFFF", i, nd.arg2);
       like_segments(s, nd.arg2, i);
       break;
-    case SB_OP_STR_OCTET_LENGTH:
-      SB_REQUIRE(nd.lit.i == 0 && nd.arg2 == 0, "STR_OCTET_LENGTH node %d takes no literal", i);
+    case SB_OP_STR_OCTET_LENGTH: case SB_OP_STR_CHAR_LENGTH:
+      SB_REQUIRE(nd.lit.i == 0 && nd.arg2 == 0, "%s node %d takes no literal", nd.op == SB_OP_STR_OCTET_LENGTH ? "STR_OCTET_LENGTH" : "STR_CHAR_LENGTH", i);
       break;
     default: SB_REQUIRE(nd.arg2 == 0, "string test node %d: arg2 %d must be 0", i, nd.arg2);
   }
@@ -136,7 +136,7 @@ StrTests strpred_compile(const sb_expr &e) {
   };
   for (int i = 0; i < e.n; i++) {
     const sb_expr_node &nd = e.nodes[i];
-    if (!strpred_is_leaf(nd.op) || nd.op == SB_OP_STR_OCTET_LENGTH) continue;
+    if (!strpred_is_leaf(nd.op) || strpred_is_length(nd.op)) continue;
     const Slice s = slice_of(e, nd);
     if (nd.op == SB_OP_STR_IN) {
       std::vector<Slice> lits;

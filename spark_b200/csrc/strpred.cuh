@@ -7,6 +7,7 @@
 //   LIKE               regexpExpressions.scala Like + StringUtils.escapeLikeRegex: the whole string matches, `%` = any run of code
 //                      points (newlines too), `_` = one code point, the escape character precedes `%`, `_` or itself only
 //   octet_length       the byte length
+//   length             UTF8String.numChars: one per step, a step being the width its lead byte declares (numBytesForFirstByte)
 //
 // The host compiles a program's literals into one blob of 32-bit words that is copied to the device once per evaluation; a node's
 // test is the word index `ref` of its descriptor in that blob:
@@ -26,7 +27,9 @@ namespace sb {
 
 constexpr uint16_t STRP_ANY = 256;
 
-inline bool strpred_is_leaf(int32_t op) { return op >= SB_OP_STR_EQ && op <= SB_OP_STR_OCTET_LENGTH; }
+inline bool strpred_is_leaf(int32_t op) { return op >= SB_OP_STR_EQ && op <= SB_OP_STR_CHAR_LENGTH; }
+// the leaves whose value is an I32 length and that take no literal
+inline bool strpred_is_length(int32_t op) { return op == SB_OP_STR_OCTET_LENGTH || op == SB_OP_STR_CHAR_LENGTH; }
 
 // host: checks string-test node `i` of `e` against `in` (a string column, the slice inside the pool, a well-formed IN list, the
 // LIKE escape rules) and returns the node's value class; SB_ERR_INVALID otherwise
@@ -61,6 +64,16 @@ __device__ __forceinline__ bool strp_equal(const uint8_t *s, const uint8_t *l, i
 }
 
 __device__ __forceinline__ bool strp_is_cont(uint8_t b) { return (b & 0xC0) == 0x80; }
+
+// UTF8String.numBytesForFirstByte: the width a lead byte declares; 1 for continuation bytes, 0xC0 / 0xC1 and 0xF5..0xFF
+__device__ __forceinline__ int strp_step(uint8_t b) { return b < 0xC2 ? 1 : b < 0xE0 ? 2 : b < 0xF0 ? 3 : b < 0xF5 ? 4 : 1; }
+
+// UTF8String.numChars of s[0..n)
+__device__ __forceinline__ int32_t strp_num_chars(const uint8_t *s, int32_t n) {
+  int32_t c = 0;
+  for (int32_t i = 0; i < n; i += strp_step(s[i])) c++;
+  return c;
+}
 
 // segment `u[0..k)` forward from p, never past n; p becomes its end
 __device__ __forceinline__ bool strp_seg_fwd(const uint16_t *u, int32_t k, const uint8_t *s, int32_t n, int32_t &p) {
@@ -125,6 +138,7 @@ __device__ __forceinline__ int64_t strpred_eval(int32_t op, uint32_t ref, const 
   const uint8_t *b = (const uint8_t *)blob;
   switch (op) {
     case SB_OP_STR_OCTET_LENGTH: return n;
+    case SB_OP_STR_CHAR_LENGTH: return strp_num_chars(s, n);
     case SB_OP_STR_IN: {
       int32_t lo = 0, hi = (int32_t)d[0] - 1;
       while (lo <= hi) {

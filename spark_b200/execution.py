@@ -25,11 +25,17 @@ import numpy as np
 
 from . import _capi as capi
 from .columnar import ColumnarBatch, Stream, _h
-from .expressions import (AggregateFunction, AttributeReference, CompiledExpr, Expression, Schema, SortOrder)
+from .expressions import (AggregateFunction, AttributeReference, CompiledExpr, CompiledStringProgram, Expression, Schema, SortOrder,
+                          StringFunction)
+
+
+def _binary_names(names, arrow_types):
+    import pyarrow as pa
+    return {n for n, t in zip(names, arrow_types) if t is not None and (pa.types.is_binary(t) or pa.types.is_large_binary(t))}
 
 
 def _schema_of(batch: ColumnarBatch) -> Schema:
-    return Schema(batch.names, [batch.column_desc(i).type for i in range(len(batch.names))])
+    return Schema(batch.names, [batch.column_desc(i).type for i in range(len(batch.names))], _binary_names(batch.names, batch.arrow_types))
 
 
 class SparkPlan:
@@ -97,6 +103,115 @@ class ProjectExec(SparkPlan):
 
 
 def _filter_project(inp: ColumnarBatch, condition, project_list, stream) -> ColumnarBatch:
+    if _has_string_function(condition) or any(_has_string_function(e) for _, e in project_list):
+        return _filter_project_strings(inp, condition, project_list, stream)
+    return _filter_project_native(inp, condition, project_list, stream)
+
+
+def _has_string_function(e) -> bool:
+    return e is not None and (isinstance(e, StringFunction) or any(_has_string_function(c) for c in e.children))
+
+
+def _hoist_string_functions(e: Expression, hidden):
+    """`e` with every string function that is an operand of a numeric or boolean node replaced by a hidden column; (name,
+    function) pairs are appended to `hidden`."""
+    import copy
+    if isinstance(e, StringFunction):
+        name = "\0sf%d" % len(hidden)
+        hidden.append((name, e))
+        return AttributeReference(name)
+    if not _has_string_function(e):
+        return e
+    e2 = copy.copy(e)
+    for attr in ("left", "right", "child"):
+        if hasattr(e2, attr):
+            setattr(e2, attr, _hoist_string_functions(getattr(e2, attr), hidden))
+    if hasattr(e2, "left"):
+        e2.children = (e2.left, e2.right)
+    elif hasattr(e2, "child"):
+        e2.children = (e2.child,)
+    return e2
+
+
+def _string_project(inp: ColumnarBatch, items, stream) -> ColumnarBatch:
+    """sb_string_project: one string column per (name, string function) of `items`, over every row of `inp`."""
+    import pyarrow as pa
+    schema = _schema_of(inp)
+    for _, e in items:
+        for a in e.references():
+            if a in schema.binary:
+                raise capi.SparkB200Error(5, "string functions over the binary column %r are not supported on the GPU" % a)
+    progs = [CompiledStringProgram(e, schema) for _, e in items]
+    arr = (capi.sb_expr * max(1, len(progs)))()
+    for i, p in enumerate(progs):
+        arr[i] = p.c
+    h = C.c_void_p()
+    capi.check(capi.load().sb_string_project(inp.handle, arr, len(progs), _h(stream), C.byref(h)))
+    return ColumnarBatch(h, [n for n, _ in items], [pa.string()] * len(items))
+
+
+def _with_hidden(inp: ColumnarBatch, hidden, stream) -> ColumnarBatch:
+    """inp ++ the hidden string columns (a new reference to inp when there are none)."""
+    if not hidden:
+        return inp.rename(inp.names)
+    h = _string_project(inp, hidden, stream)
+    try:
+        return inp.zip(h)
+    finally:
+        h.close()
+
+
+def _filter_project_strings(inp: ColumnarBatch, condition, project_list, stream) -> ColumnarBatch:
+    """Filter + projection when string functions take part.  A string function inside the condition is materialised as a hidden
+    column over all rows, the condition runs over inp ++ hidden, and the hidden columns are dropped with the rows.  The projections
+    then run over the surviving rows only: string-valued outputs through sb_string_project, the rest through sb_filter_project (a
+    string function inside them hoisted the same way), joined with sb_table_zip in the projection's order."""
+    cur = inp.rename(inp.names)
+    try:
+        if condition is not None:
+            hidden = []
+            cond = _hoist_string_functions(condition, hidden)
+            wide = _with_hidden(cur, hidden, stream)
+            try:
+                kept = _filter_project_native(wide, cond, [(n, AttributeReference(n)) for n in inp.names], stream)
+            finally:
+                wide.close()
+            cur.close()
+            cur = kept
+        if not project_list:
+            return _filter_project_native(cur, None, [], stream)
+        strings = [(i, n, e) for i, (n, e) in enumerate(project_list) if isinstance(e, StringFunction)]
+        others = [(i, n, e) for i, (n, e) in enumerate(project_list) if not isinstance(e, StringFunction)]
+        parts = []
+        try:
+            if others:
+                hidden = []
+                exprs = [("\0p%d" % i, _hoist_string_functions(e, hidden)) for i, _, e in others]
+                wide = _with_hidden(cur, hidden, stream)
+                try:
+                    parts.append(_filter_project_native(wide, None, exprs, stream))
+                finally:
+                    wide.close()
+            if strings:
+                parts.append(_string_project(cur, [("\0p%d" % i, e) for i, _, e in strings], stream))
+            out = parts[0] if len(parts) == 1 else parts[0].zip(parts[1])
+            if len(parts) == 2:
+                parts[0].close()
+                parts[1].close()
+            parts = [out]
+            sel = out.select(["\0p%d" % i for i in range(len(project_list))])
+            try:
+                return sel.rename([n for n, _ in project_list])
+            finally:
+                sel.close()
+        finally:
+            for b in parts:
+                b.close()
+    finally:
+        cur.close()
+
+
+def _filter_project_native(inp: ColumnarBatch, condition, project_list, stream) -> ColumnarBatch:
     lib = capi.load()
     schema = _schema_of(inp)
     pred = CompiledExpr(condition, schema) if condition is not None else None
@@ -692,7 +807,8 @@ def probe_join(rel: HashedRelation, probe: ColumnarBatch, keys, joinType, stream
     p_types = [probe.arrow_types[i] for i in p_sel]
     if condition is not None:
         # the residual condition sees the joined row as the kernels lay it out: streamed columns ++ build columns
-        schema = Schema(probe.names + rel.names, [probe.column_desc(i).type for i in range(len(probe.names))] + rel.types)
+        schema = Schema(probe.names + rel.names, [probe.column_desc(i).type for i in range(len(probe.names))] + rel.types,
+                        _binary_names(probe.names + rel.names, probe.arrow_types + rel.arrow_types))
         ce = CompiledExpr(condition, schema)
         capi.check(lib.sb_join_probe_condition(rel.handle, probe.handle, arr, len(idx), capi.SB_JOIN[joinType], C.byref(ce.c), _h(stream), C.byref(h)))
     elif probe_filter is not None or probe_out is not None or rel.out_cols is not None or runtime_filters:

@@ -24,9 +24,10 @@ _OUT_OF_VT = {VT_BOOL: capi.SB_BOOL, VT_I32: capi.SB_INT32, VT_I64: capi.SB_INT6
 class Schema:
     """names + physical sb types of an operator's input (the `output: Seq[Attribute]` of a SparkPlan)."""
 
-    def __init__(self, names, types):
+    def __init__(self, names, types, binary=()):
         self.names = list(names)
         self.types = list(types)
+        self.binary = set(binary)        # SB_STRING columns whose values are binary, not strings (Length counts their bytes)
 
     def index(self, name):
         try:
@@ -270,9 +271,9 @@ class _Comparison(Expression):
     def _string_sides(self):
         """(column, literal bytes, flipped) when this compares a string column with a string literal, else None."""
         l, r = self.left, self.right
-        if isinstance(r, AttributeReference) and _is_str_lit(l):
+        if isinstance(r, (AttributeReference, StringFunction)) and _is_str_lit(l):
             return r, _utf8(l.value), True
-        if isinstance(l, AttributeReference) and _is_str_lit(r):
+        if isinstance(l, (AttributeReference, StringFunction)) and _is_str_lit(r):
             return l, _utf8(r.value), False
         return None
 
@@ -406,6 +407,8 @@ def _is_str_lit(e) -> bool:
 
 
 def _string_col(c, schema) -> int:
+    if isinstance(c, StringFunction):
+        raise TypeError("%s: a string function inside a numeric program is evaluated first (execution.py hoists it into a column)" % c.name)
     i = schema.index(c.name)
     if schema.types[i] != capi.SB_STRING:
         raise TypeError("%r is not a string column" % c.name)
@@ -417,8 +420,8 @@ class _StringTest(Expression):
     name = None
 
     def __init__(self, child, literal):
-        if not isinstance(child, AttributeReference):
-            raise TypeError("string tests take a string column")
+        if not isinstance(child, (AttributeReference, StringFunction)):
+            raise TypeError("string tests take a string column or a string function")
         self.child, self.literal = child, _utf8(literal)
         self.children = (child,)
 
@@ -494,6 +497,228 @@ class OctetLength(_StringTest):
 
     def sexpr(self):
         return ("octet_length", self.child.sexpr())
+
+
+class Length(OctetLength):
+    """length(str): the code points, counted as UTF8String.numChars counts them (one per lead byte); over a binary column the bytes
+    (stringExpressions.scala Length: `case BinaryType => value.length`)."""
+    op, name = "STR_CHAR_LENGTH", "length"
+
+    def emit(self, schema, out):
+        i = _string_col(self.child, schema)
+        out.append(_node("STR_OCTET_LENGTH" if self.child.name in schema.binary else self.op, VT_I32, i))
+
+    def sexpr(self):
+        return ("length", self.child.sexpr())
+
+
+# ---- string-producing functions (stringExpressions.scala, collectionOperations.scala Concat) ----------------------------------
+# Their value is a string, so they are programs of their own (SB_OP_SF_*, sb_string_project) rather than nodes of a numeric one.
+# Positions, lengths and pad lengths are int literals; trim sets, pads and separators string literals; a None among them is a NULL
+# literal and gives the function's NULL answer.  String operands are string columns, string literals or other string functions.
+_INT_MAX = 2 ** 31 - 1
+_ABSENT = object()
+
+
+def _int_arg(v, what):
+    if isinstance(v, Literal):
+        v = v.value
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, int) or not -2 ** 31 <= v < 2 ** 31:
+        raise capi.SparkB200Error(5, "%s must be an int literal (got %r)" % (what, v))
+    return v
+
+
+def _str_arg(v, what):
+    if isinstance(v, Literal):
+        v = v.value
+    if v is None:
+        return None
+    if not isinstance(v, (str, bytes)):
+        raise capi.SparkB200Error(5, "%s must be a string literal (got %r)" % (what, v))
+    return _utf8(v)
+
+
+def _string_operand(e):
+    if isinstance(e, (str, bytes)) or e is None:
+        return Literal(e, 0)
+    if isinstance(e, Literal) and (e.value is None or isinstance(e.value, (str, bytes))):
+        return Literal(e.value, 0)
+    if isinstance(e, (AttributeReference, StringFunction)):
+        return e
+    raise capi.SparkB200Error(5, "string functions take string columns, string literals or string functions (got %r)" % (e,))
+
+
+def _emit_sf_operand(e, schema, out):
+    if isinstance(e, StringFunction):
+        e.emit_sf(schema, out)
+    elif isinstance(e, Literal):
+        if e.value is None:
+            out.append(_node("SF_LIT", 0, arg2=1))
+        else:
+            out.append(_node("SF_LIT", 0, lit_i=_pool(out).slice(_utf8(e.value))))
+    else:
+        out.append(_node("SF_COL", 0, _string_col(e, schema)))
+
+
+def _sexpr_operand(e):
+    return ("lit", e.value, bytes) if isinstance(e, Literal) else e.sexpr()
+
+
+class StringFunction(Expression):
+    name = None
+
+    def vtype(self, schema):
+        return 0
+
+    def emit(self, schema, out):
+        raise TypeError("%s yields a string: it is evaluated by sb_string_project, not inside a numeric program" % self.name)
+
+    def emit_sf(self, schema, out):
+        raise NotImplementedError
+
+
+class Substring(StringFunction):
+    """substring(str, pos[, len]) (UTF8String.substringSQL); len omitted = Integer.MAX_VALUE."""
+    name = "substring"
+
+    def __init__(self, child, pos, len=_INT_MAX):
+        self.child = _string_operand(child)
+        self.children = (self.child,)
+        self.pos, self.len = _int_arg(pos, "substring position"), _int_arg(len, "substring length")
+
+    def emit_sf(self, schema, out):
+        if self.pos is None or self.len is None:
+            out.append(_node("SF_LIT", 0, arg2=1))
+            return
+        _emit_sf_operand(self.child, schema, out)
+        out.append(_node("SF_SUBSTRING", 0, self.pos, arg2=self.len))
+
+    def sexpr(self):
+        return ("substring", _sexpr_operand(self.child), self.pos, self.len)
+
+
+class Concat(StringFunction):
+    """concat(s1, s2, ...): NULL if any input is NULL."""
+    name = "concat"
+
+    def __init__(self, *children):
+        self.children = tuple(_string_operand(c) for c in children)
+
+    def emit_sf(self, schema, out):
+        if not self.children:
+            out.append(_node("SF_LIT", 0, lit_i=_pool(out).slice(b"")))
+            return
+        for c in self.children:
+            _emit_sf_operand(c, schema, out)
+        out.append(_node("SF_CONCAT", 0, len(self.children)))
+
+    def sexpr(self):
+        return ("concat",) + tuple(_sexpr_operand(c) for c in self.children)
+
+
+class ConcatWs(StringFunction):
+    """concat_ws(sep, s1, s2, ...): NULL inputs are skipped; a NULL separator gives NULL."""
+    name = "concat_ws"
+
+    def __init__(self, sep, *children):
+        self.sep = _str_arg(sep, "concat_ws separator")
+        self.children = tuple(_string_operand(c) for c in children)
+
+    def emit_sf(self, schema, out):
+        if self.sep is None:
+            out.append(_node("SF_LIT", 0, arg2=1))
+        elif not self.children:
+            out.append(_node("SF_LIT", 0, lit_i=_pool(out).slice(b"")))
+        else:
+            for c in self.children:
+                _emit_sf_operand(c, schema, out)
+            out.append(_node("SF_CONCAT_WS", 0, len(self.children), lit_i=_pool(out).slice(self.sep)))
+
+    def sexpr(self):
+        return ("concat_ws", self.sep) + tuple(_sexpr_operand(c) for c in self.children)
+
+
+class _Trim(StringFunction):
+    op = None
+
+    def __init__(self, srcStr, trimStr=_ABSENT):
+        self.child = _string_operand(srcStr)
+        self.children = (self.child,)
+        self.given = trimStr is not _ABSENT
+        self.trim = _str_arg(trimStr, "trim string") if self.given else None
+
+    def emit_sf(self, schema, out):
+        if self.given and self.trim is None:
+            out.append(_node("SF_LIT", 0, arg2=1))
+            return
+        _emit_sf_operand(self.child, schema, out)
+        if self.given:
+            out.append(_node(self.op, 0, 1, lit_i=_pool(out).slice(self.trim)))
+        else:
+            out.append(_node(self.op, 0, 0))
+
+    def sexpr(self):
+        return (self.name, _sexpr_operand(self.child), self.trim if self.given else ())
+
+
+class StringTrim(_Trim):
+    """trim(str) removes ASCII spaces; trim(str, trimStr) every code point that occurs in trimStr, from both ends."""
+    op, name = "SF_TRIM", "trim"
+
+
+class StringTrimLeft(_Trim):
+    op, name = "SF_LTRIM", "ltrim"
+
+
+class StringTrimRight(_Trim):
+    op, name = "SF_RTRIM", "rtrim"
+
+
+class _Pad(StringFunction):
+    op = None
+
+    def __init__(self, str, len, pad=" "):
+        self.child = _string_operand(str)
+        self.children = (self.child,)
+        self.len = _int_arg(len, "pad length")
+        self.pad = _str_arg(pad, "pad")
+
+    def emit_sf(self, schema, out):
+        if self.len is None or self.pad is None:
+            out.append(_node("SF_LIT", 0, arg2=1))
+            return
+        _emit_sf_operand(self.child, schema, out)
+        out.append(_node(self.op, 0, self.len, lit_i=_pool(out).slice(self.pad)))
+
+    def sexpr(self):
+        return (self.name, _sexpr_operand(self.child), self.len, self.pad)
+
+
+class StringLPad(_Pad):
+    """lpad(str, len, pad): padding counted in code points."""
+    op, name = "SF_LPAD", "lpad"
+
+
+class StringRPad(_Pad):
+    op, name = "SF_RPAD", "rpad"
+
+
+class CompiledStringProgram:
+    """Owns the ctypes arrays behind one string-producing sb_expr (SB_OP_SF_* nodes, out_type SB_STRING)."""
+
+    def __init__(self, expr: Expression, schema: Schema):
+        nodes = _Program()
+        _emit_sf_operand(_string_operand(expr), schema, nodes)
+        self.arr = (capi.sb_expr_node * len(nodes))(*nodes)
+        self.c = capi.sb_expr()
+        self.c.nodes = C.cast(self.arr, C.POINTER(capi.sb_expr_node))
+        self.c.n = len(nodes)
+        self.pool = (C.c_uint8 * max(1, len(nodes.pool))).from_buffer_copy(bytes(nodes.pool) or b"\0")
+        self.c.bytes = C.cast(self.pool, C.c_void_p) if nodes.pool else None
+        self.c.nbytes = len(nodes.pool)
+        self.c.out_type = capi.SB_STRING
 
 
 class CompiledExpr:
