@@ -202,7 +202,9 @@ typedef struct sb_column_chunk {
   const sb_page *pages;
   int64_t dict_offset;              /* PLAIN dictionary values, or -1 */
   int32_t dict_count;
-  int32_t pad;
+  int32_t value_multiplier;         /* 0 or 1: values as stored.  Else each decoded INT64 value is multiplied by it (wrapping), in
+                                       every encoding: 1000 reads a TIMESTAMP(MILLIS) column as SB_TIMESTAMP microseconds, the
+                                       conversion of the reference's LongAsMicrosUpdater */
 } sb_column_chunk;
 
 /* host only (no device): page descriptors of a column chunk lying in a Parquet file: Thrift compact PageHeader walk (data page
@@ -236,6 +238,8 @@ typedef struct sb_page_span {       /* one page of a chunk as it lies in the fil
 typedef struct sb_compressed_chunk {
   int32_t type, scale, physical_type, codec;   /* codec: SB_CODEC_* */
   int32_t max_def_level, npages;
+  int32_t value_multiplier;         /* as sb_column_chunk.value_multiplier (0: values as stored) */
+  int32_t pad;
   const uint8_t *data;              /* HOST bytes of the chunk as they lie in the file, headers included */
   int64_t data_bytes;
   const sb_page_span *spans;        /* from sb_parquet_page_spans, the dictionary page included */
@@ -256,7 +260,9 @@ int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int32_t ncols, 
 
 /* write-side twin (tests, bench.py): one NULL-free fixed-width column -> a column chunk on the device (out_chunk: one SB_INT8
  * column of bytes) + page descriptors on the host.  dictionary: one-column table of the distinct values in ascending order,
- * or NULL for PLAIN pages. */
+ * or NULL for PLAIN pages.  For an SB_FLOAT32 / SB_FLOAT64 column the dictionary holds the distinct BIT PATTERNS as an SB_INT32 /
+ * SB_INT64 column in ascending signed order, so that -0.0 and every NaN payload keep an entry of their own and decode to the bits
+ * they were written with (a Parquet dictionary need not be in numeric order). */
 int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *dictionary, int64_t page_rows, sb_stream *s, sb_table **out_chunk,
                    sb_page *out_pages, int32_t pages_cap, int32_t *out_npages, int64_t *out_dict_offset, int32_t *out_dict_count);
 

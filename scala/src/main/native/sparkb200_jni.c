@@ -627,6 +627,7 @@ NATIVE(jlong, scanDecode)(JNIEnv *env, jclass c, jintArray types, jintArray scal
     chunks[i].pages = owned[i];
     chunks[i].dict_offset = flat[6 * npages + 0];
     chunks[i].dict_count = (int32_t)flat[6 * npages + 1];
+    chunks[i].value_multiplier = 0;   /* values as stored: the page tables carry no timestamp unit */
     (*env)->ReleaseLongArrayElements(env, pt, flat, JNI_ABORT);
   }
   sb_table *out = NULL;
@@ -709,6 +710,7 @@ NATIVE(jlong, scanDecodeCompressed)(JNIEnv *env, jclass c, jintArray types, jint
     chunks[i].data = (const uint8_t *)(intptr_t)ad[i];
     chunks[i].data_bytes = sz[i];
     chunks[i].spans = owned[i];
+    chunks[i].value_multiplier = 0;
     (*env)->ReleaseLongArrayElements(env, st, flat, JNI_ABORT);
   }
   sb_table *out = NULL;

@@ -30,6 +30,11 @@ SB_AGG_MODE = dict(partial=1, final=2, complete=3, partial_merge=4)
 SB_JOIN = dict(inner=0, left_outer=1, left_semi=2, left_anti=3, full_outer=4, build_outer=5, existence=6, left_anti_null_aware=7)
 SB_UNIQUE_ID_BYTES = 128
 
+def decimal_type(precision, scale):
+    """sb_column.scale word of a decimal column: SB_DECIMAL_TYPE(precision, scale)"""
+    return (precision << 8) | scale
+
+
 TYPE_WIDTH = {SB_BOOL: 1, SB_INT8: 1, SB_INT16: 2, SB_INT32: 4, SB_INT64: 8, SB_FLOAT32: 4, SB_FLOAT64: 8,
               SB_DATE32: 4, SB_TIMESTAMP: 8, SB_DECIMAL64: 8, SB_STRING: 0, SB_DECIMAL128: 16}
 
@@ -46,7 +51,7 @@ class sb_page(C.Structure):
 
 class sb_column_chunk(C.Structure):
     _fields_ = [("type", C.c_int32), ("scale", C.c_int32), ("physical_type", C.c_int32), ("npages", C.c_int32), ("data", C.c_void_p),
-                ("data_bytes", C.c_int64), ("pages", C.POINTER(sb_page)), ("dict_offset", C.c_int64), ("dict_count", C.c_int32), ("pad", C.c_int32)]
+                ("data_bytes", C.c_int64), ("pages", C.POINTER(sb_page)), ("dict_offset", C.c_int64), ("dict_count", C.c_int32), ("value_multiplier", C.c_int32)]
 
 
 class sb_page_span(C.Structure):
@@ -57,7 +62,8 @@ class sb_page_span(C.Structure):
 
 class sb_compressed_chunk(C.Structure):
     _fields_ = [("type", C.c_int32), ("scale", C.c_int32), ("physical_type", C.c_int32), ("codec", C.c_int32),
-                ("max_def_level", C.c_int32), ("npages", C.c_int32), ("data", C.c_void_p), ("data_bytes", C.c_int64),
+                ("max_def_level", C.c_int32), ("npages", C.c_int32), ("value_multiplier", C.c_int32), ("pad", C.c_int32),
+                ("data", C.c_void_p), ("data_bytes", C.c_int64),
                 ("spans", C.POINTER(sb_page_span))]
 
 

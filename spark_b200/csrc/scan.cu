@@ -52,7 +52,7 @@ struct ColTask {
   int32_t dict_count;
   int32_t phys_width;        // 0 BOOLEAN (bit-packed), 4, 8
   int32_t out_width;         // 1, 2, 4, 8
-  int32_t pad;
+  int32_t mul;               // sb_column_chunk.value_multiplier (<= 1: values as stored)
 };
 
 __device__ __forceinline__ uint64_t load_le(const uint8_t *p, int nbytes) {
@@ -67,6 +67,14 @@ __device__ __forceinline__ void store_value(void *out, int width, int64_t i, uin
     case 4: ((uint32_t *)out)[i] = (uint32_t)v; break;
     default: ((uint64_t *)out)[i] = v; break;
   }
+}
+
+// a physical value as the column holds it: INT32 sign-extended into a decimal64, then the unit multiplier (TIMESTAMP(MILLIS) ->
+// microseconds; wraps like the reference's long arithmetic would before its overflow check)
+__device__ __forceinline__ uint64_t column_value(uint64_t v, int pw, int ow, int32_t mul) {
+  if (pw == 4 && ow == 8) v = (uint64_t)(int64_t)(int32_t)v;   // decimal(p <= 9) stored as INT32
+  if (mul > 1) v *= (uint64_t)mul;
+  return v;
 }
 
 // unsigned LEB128 at p[pos] (bounded by nbytes); returns the value, *len = bytes consumed
@@ -472,7 +480,22 @@ __device__ int64_t count_valid(const uint8_t *vb, int64_t n) {
   return (int64_t)tot;
 }
 
-__global__ void __launch_bounds__(SCAN_THREADS) scan_decode_kernel(const PageTask *__restrict__ pages, const ColTask *__restrict__ cols, int nparts) {
+// RLE_DICTIONARY values of a page: [bit width][hybrid runs of dictionary indices].  SCALED (TIMESTAMP(MILLIS)) is a template
+// constant so that the other pages keep the hot loop they have without a multiplier.
+template <bool SCALED>
+__device__ __forceinline__ void dict_values(const PageTask &pg, const ColTask &c, void *dense, int part, int nparts) {
+  const int bw = pg.values_bytes > 0 ? pg.values[0] : 0;
+  const uint8_t *dict = c.dict;
+  const int pw = c.phys_width, ow = c.out_width, dcount = c.dict_count, mul = SCALED ? c.mul : 0;
+  hybrid_decode(pg.values + 1, pg.values_bytes - 1, bw, pg.num_values, part, nparts, [&](int64_t i, uint64_t idx) {
+    uint64_t v = 0;
+    if ((int64_t)idx < dcount) v = column_value(pw == 0 ? dict[idx] : load_le(dict + idx * pw, pw), pw, ow, mul);
+    store_value(dense, ow, i, v);
+  });
+}
+
+// (4 blocks per SM: the register budget the kernel had before the TIMESTAMP(MILLIS) path, at no spill)
+__global__ void __launch_bounds__(SCAN_THREADS, 4) scan_decode_kernel(const PageTask *__restrict__ pages, const ColTask *__restrict__ cols, int nparts) {
   const PageTask pg = pages[blockIdx.x / nparts];
   int part = blockIdx.x % nparts;
   const ColTask c = cols[pg.col];
@@ -497,7 +520,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_decode_kernel(const PageTas
     } else {
       const int pw = c.phys_width;
       const int64_t avail = pg.values_bytes / pw < n ? pg.values_bytes / pw : n;
-      if (pw == ow && ((((uintptr_t)pg.values) | ((uintptr_t)dense)) & 15) == 0) {   // straight copy, 16 bytes per thread
+      if (pw == ow && c.mul <= 1 && ((((uintptr_t)pg.values) | ((uintptr_t)dense)) & 15) == 0) {   // straight copy, 16 bytes per thread
         const int64_t bytes = avail * pw, vec = bytes >> 4;
         const uint4 *s4 = (const uint4 *)pg.values;
         uint4 *d4 = (uint4 *)dense;
@@ -505,25 +528,17 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_decode_kernel(const PageTas
         for (int64_t i = (vec << 4) + tid; i < bytes; i += SCAN_THREADS) ((uint8_t *)dense)[i] = pg.values[i];
       } else {
         for (int64_t i = tid; i < avail; i += SCAN_THREADS) {
-          uint64_t v = load_le(pg.values + i * pw, pw);
-          if (pw == 4 && ow == 8) v = (uint64_t)(int64_t)(int32_t)v;   // decimal(p <= 9) stored as INT32
-          store_value(dense, ow, i, v);
+          store_value(dense, ow, i, column_value(load_le(pg.values + i * pw, pw), pw, ow, c.mul));
         }
       }
     }
   } else if (pg.encoding == SB_ENC_RLE_BOOLEAN) {   // BOOLEAN values as RLE (data page V2 writers): [4-byte length][hybrid, bit width 1]
     if (pg.values_bytes > 4)
       hybrid_decode(pg.values + 4, pg.values_bytes - 4, 1, n, 0, 1, [&](int64_t i, uint64_t v) { ((uint8_t *)dense)[i] = (uint8_t)(v & 1); });
-  } else {   // RLE_DICTIONARY: [bit width][hybrid runs of dictionary indices]
-    const int bw = pg.values_bytes > 0 ? pg.values[0] : 0;
-    const uint8_t *dict = c.dict;
-    const int pw = c.phys_width, dcount = c.dict_count;
-    hybrid_decode(pg.values + 1, pg.values_bytes - 1, bw, n, part, nparts, [&](int64_t i, uint64_t idx) {
-      uint64_t v = 0;
-      if ((int64_t)idx < dcount) v = pw == 0 ? dict[idx] : load_le(dict + idx * pw, pw);
-      if (pw == 4 && ow == 8) v = (uint64_t)(int64_t)(int32_t)v;
-      store_value(dense, ow, i, v);
-    });
+  } else if (c.mul > 1) {   // RLE_DICTIONARY: [bit width][hybrid runs of dictionary indices]
+    dict_values<true>(pg, c, dense, part, nparts);
+  } else {
+    dict_values<false>(pg, c, dense, part, nparts);
   }
   if (!page_nullable) return;
   __syncthreads();
@@ -540,12 +555,11 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_delta_kernel(const PageTask
   uint8_t *vb = c.valid_bytes ? c.valid_bytes + pg.row_start : nullptr;
   const bool page_nullable = pg.def != nullptr && pg.def_bytes > 0;
   if (vb) decode_validity(pg, vb, page_nullable);
-  const int ow = c.out_width, pw = c.phys_width;
+  const int ow = c.out_width, pw = c.phys_width, mul = c.mul;
   void *dst_page = (uint8_t *)c.out + pg.row_start * ow;
   void *dense = page_nullable ? (void *)(c.dense + pg.row_start * ow) : dst_page;
   dbp_decode(pg.values, pg.values_bytes, n, [&](int64_t i, uint64_t v) {   // 64-bit running sum, truncated to the column's width
-    if (pw == 4 && ow == 8) v = (uint64_t)(int64_t)(int32_t)v;
-    store_value(dense, ow, i, v);
+    store_value(dense, ow, i, column_value(v, pw, ow, mul));
   });
   if (!page_nullable) return;
   __syncthreads();
@@ -1197,6 +1211,8 @@ static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols
         SB_REQUIRE(ow > 0, "column chunk %d: string columns are decoded from physical type BYTE_ARRAY only", ci);
         SB_REQUIRE(pw == 0 ? ch.type == SB_BOOL : (pw == 8 ? ow == 8 : (ow <= 4 || ch.type == SB_DECIMAL64)), "column chunk %d: physical type %d cannot feed column type %d", ci,
                    ch.physical_type, ch.type);
+        SB_REQUIRE(ch.value_multiplier >= 0 && (ch.value_multiplier <= 1 || (ch.physical_type == SB_PHYS_INT64 && (ch.type == SB_TIMESTAMP || ch.type == SB_INT64))),
+                   "column chunk %d: value multiplier %d applies to INT64 timestamp / long columns only", ci, ch.value_multiplier);
       }
       int64_t rows = 0;
       bool nullable = false;
@@ -1292,6 +1308,7 @@ static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols
       }
       ct.phys_width = pw;
       ct.out_width = ow;
+      ct.mul = ch.value_multiplier;
       int64_t row = 0;
       for (int p = 0; p < ch.npages; p++) {
         const sb_page &pg = ch.pages[p];
@@ -1465,6 +1482,7 @@ extern "C" int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int3
     d.type = ch.type;
     d.scale = ch.scale;
     d.physical_type = ch.physical_type;
+    d.value_multiplier = ch.value_multiplier;
     d.data = images[ci]->as<uint8_t>();   // the image (device); scan_decode_chunks reads it through device_bytes only
     d.data_bytes = img_bytes[ci];
     d.dict_offset = -1;
@@ -1500,7 +1518,8 @@ extern "C" int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int3
 
 // Write-side twin for tests and bench.py: encodes one fixed-width column of `t` as a column chunk in the layout
 // sb_scan_decode reads.  dictionary == nullptr: PLAIN pages.  Otherwise `dictionary` is a one-column table holding the
-// column's distinct values in ascending order (e.g. sb_hash_aggregate with no aggregates + sb_sort): the chunk is
+// column's distinct values in ascending order (e.g. sb_hash_aggregate with no aggregates + sb_sort; a float column's distinct
+// bit patterns as integers, so -0.0 and each NaN payload are entries of their own): the chunk is
 // [PLAIN dictionary values][pages of bit-packed indices].  The chunk stays on the device (out_chunk: one SB_INT8 column of
 // bytes); page descriptors come back on the host.  No NULLs (definition levels are not written).
 extern "C" int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *dictionary, int64_t page_rows, sb_stream *s, sb_table **out_chunk,
@@ -1536,7 +1555,10 @@ extern "C" int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *di
     *out_dict_offset = -1;
     *out_dict_count = 0;
   } else {
-    SB_REQUIRE(dictionary->cols.size() == 1 && dictionary->cols[0].type == c.type && !dictionary->cols[0].validity, "dictionary must be one NULL-free column of the column's type");
+    // floats: the dictionary holds bit patterns (integers of the same width), searched in signed integer order
+    const int32_t dict_type = c.type == SB_FLOAT32 ? SB_INT32 : c.type == SB_FLOAT64 ? SB_INT64 : c.type;
+    SB_REQUIRE(dictionary->cols.size() == 1 && dictionary->cols[0].type == dict_type && !dictionary->cols[0].validity,
+               "dictionary must be one NULL-free column of type %d (the column's type; the bit patterns of a float column)", dict_type);
     const int64_t dcount = dictionary->nrows;
     SB_REQUIRE(dcount >= 1 && dcount <= (1 << 24), "dictionary of %lld entries", (long long)dcount);
     int bw = 0;
@@ -1568,9 +1590,7 @@ extern "C" int sb_scan_encode(const sb_table *t, int32_t col, const sb_table *di
       switch (c.type) {
         case SB_INT8: encode_dict_pages_kernel<int8_t><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const int8_t *)c.d(), n, (const int8_t *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
         case SB_INT16: encode_dict_pages_kernel<int16_t><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const int16_t *)c.d(), n, (const int16_t *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
-        case SB_INT32: case SB_DATE32: encode_dict_pages_kernel<int32_t><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const int32_t *)c.d(), n, (const int32_t *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
-        case SB_FLOAT32: encode_dict_pages_kernel<float><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const float *)c.d(), n, (const float *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
-        case SB_FLOAT64: encode_dict_pages_kernel<double><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const double *)c.d(), n, (const double *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
+        case SB_INT32: case SB_DATE32: case SB_FLOAT32: encode_dict_pages_kernel<int32_t><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const int32_t *)c.d(), n, (const int32_t *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
         default: encode_dict_pages_kernel<int64_t><<<(unsigned)npages, SCAN_THREADS, 0, st>>>((const int64_t *)c.d(), n, (const int64_t *)dv, (int32_t)dcount, bw, page_rows, page_stride, pages_base); break;
       }
       SB_LAUNCH_CHECK();
