@@ -246,7 +246,8 @@ typedef struct sb_compressed_chunk {
 } sb_compressed_chunk;
 
 /* host only (no device): the spans of every dictionary and data page of a chunk.  Checks that each body lies inside the chunk,
- * that the level bytes fit the page, that a dictionary page is PLAIN and that there are no repetition levels.  Whether a page is
+ * that no size or value count is negative, that the level bytes fit the page, that a dictionary page is PLAIN and that there
+ * are no repetition levels (sb_parquet_chunk_pages walks the headers with the same checks).  Whether a page is
  * compressed comes from the codec (the footer's), not from its two sizes.  A codec other than SB_CODEC_UNCOMPRESSED or
  * SB_CODEC_SNAPPY (GZIP, LZO, BROTLI, LZ4, ZSTD, LZ4_RAW) -> SB_ERR_UNSUPPORTED. */
 int sb_parquet_page_spans(const uint8_t *chunk, int64_t nbytes, int32_t codec, int32_t max_def_level, sb_page_span *out, int32_t cap,

@@ -970,8 +970,7 @@ void check_data_page_header(const PageHeader &h, int32_t max_def_level) {
 
 // Levels and values of one data page whose body (as decoded) is [body, body + body_bytes) of the chunk: a V1 page of an optional
 // column starts with the 4-byte length of its definition levels (`len4`; nullptr when the body is shorter), a V2 page gives the
-// length in its header.  Both page walkers call it (and then check_delta_header on the values), so a page is refused with the same
-// message whether or not it was compressed.
+// length in its header.
 void data_page_sections(sb_page &pg, bool v1, int32_t max_def_level, int32_t v2_def_len, int64_t body, int64_t body_bytes, const uint8_t *len4) {
   int64_t vpos = body;
   const int64_t vend = body + body_bytes;
@@ -994,54 +993,112 @@ void data_page_sections(sb_page &pg, bool v1, int32_t max_def_level, int32_t v2_
   pg.values_offset = vpos;
   pg.values_bytes = vend - vpos;
 }
-}  // namespace
 
-// Host only (no device needed): walks the pages of one column chunk as it lies in a Parquet file (the byte range
-// [dictionary_page_offset or data_page_offset, + total_compressed_size) of the column's metadata) and fills the descriptors
-// sb_scan_decode takes.  max_def_level: 0 for a required column, 1 for an optional one.
-extern "C" int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int32_t max_def_level, sb_page *out_pages, int32_t pages_cap,
-                                      int32_t *out_npages, int64_t *out_dict_offset, int32_t *out_dict_count) {
-  SB_API_BEGIN
-  SB_REQUIRE(chunk && out_pages && out_npages && out_dict_offset && out_dict_count && nbytes >= 0, "null argument");
+// The page header walk of a chunk as it lies in a file ([dictionary_page_offset or data_page_offset, + total_compressed_size) of
+// the column's metadata): calls page(span) for each dictionary and data page that passes the checks of every path, in order, and
+// skips INDEX_PAGE and unknown types.  `cap` bounds the pages passed on (data pages only unless cap_dictionary).
+// refuse_compressed: a page whose two sizes differ is SB_ERR_UNSUPPORTED unless it is a V2 page marked uncompressed.
+template <class Page>
+void walk_pages(const uint8_t *chunk, int64_t nbytes, int32_t codec, int32_t max_def_level, bool refuse_compressed, int32_t cap,
+                bool cap_dictionary, Page page) {
   SB_REQUIRE(max_def_level == 0 || max_def_level == 1, "nested schemas are not supported (max definition level %d)", max_def_level);
-  int32_t np = 0;
-  *out_dict_offset = -1;
-  *out_dict_count = 0;
-  int64_t pos = 0;
-  while (pos < nbytes) {
+  int32_t counted = 0;
+  for (int64_t pos = 0, next; pos < nbytes; pos = next) {
     Thrift t{chunk + pos, chunk + nbytes};
     PageHeader h;
     if (!read_page_header(t, h)) fail(SB_ERR_INVALID, "malformed Parquet page header at byte %lld of the column chunk", (long long)pos);
     const int64_t body = t.p - chunk;
-    if (h.compressed != h.uncompressed && !(h.is_v2 && !h.v2_compressed))
+    const bool stored = h.is_v2 && !h.v2_compressed;
+    if (refuse_compressed && h.compressed != h.uncompressed && !stored)
       fail(SB_ERR_UNSUPPORTED, "compressed Parquet pages are not decoded on this path (page at byte %lld: %d -> %d bytes)", (long long)pos,
            h.compressed, h.uncompressed);
-    SB_REQUIRE(body + h.compressed <= nbytes, "Parquet page at byte %lld overruns the column chunk", (long long)pos);
-    if (h.type == 2) {   // DICTIONARY_PAGE
+    SB_REQUIRE(h.compressed >= 0 && h.uncompressed >= 0 && body + h.compressed <= nbytes, "Parquet page at byte %lld overruns the column chunk",
+               (long long)pos);
+    next = body + h.compressed;
+    if (h.type != 0 && h.type != 2 && h.type != 3) continue;
+    if (h.type != 2 || cap_dictionary) {
+      SB_REQUIRE(counted < cap, "more than %d pages in the column chunk", cap);
+      counted++;
+    }
+    SB_REQUIRE(h.num_values >= 0, "Parquet page at byte %lld has a negative value count (%d)", (long long)pos, h.num_values);
+    sb_page_span sp;
+    memset(&sp, 0, sizeof(sp));
+    sp.page_type = h.type;
+    sp.num_values = h.num_values;
+    sp.body_offset = body;
+    sp.header_bytes = (int32_t)(body - pos);
+    sp.compressed_bytes = h.compressed;
+    sp.uncompressed_bytes = h.uncompressed;
+    sp.values_compressed = codec != SB_CODEC_UNCOMPRESSED && !stored;
+    if (h.type == 2) {
       SB_REQUIRE(h.encoding == 0 || h.encoding == 2, "dictionary page encoding %d is not PLAIN", h.encoding);
-      *out_dict_offset = body;
-      *out_dict_count = h.num_values;
-    } else if (h.type == 0 || h.type == 3) {   // DATA_PAGE / DATA_PAGE_V2
-      SB_REQUIRE(np < pages_cap, "more than %d pages in the column chunk", pages_cap);
-      sb_page &pg = out_pages[np++];
-      memset(&pg, 0, sizeof(pg));
-      pg.encoding = page_encoding(h.encoding);
-      pg.num_values = h.num_values;
+      sp.encoding = SB_ENC_PLAIN;
+    } else {
+      sp.encoding = page_encoding(h.encoding);
       check_data_page_header(h, max_def_level);
-      data_page_sections(pg, h.type == 0, max_def_level, h.def_len, body, h.compressed, h.compressed >= 4 ? chunk + body : nullptr);
-      if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED) check_delta_header(chunk + pg.values_offset, pg.values_bytes, pg.encoding, h.num_values, np - 1, pos);
-    }   // INDEX_PAGE and unknown page types are skipped
-    pos = body + h.compressed;
+      if (h.type == 3) sp.levels_bytes = h.def_len;
+    }
+    SB_REQUIRE(sp.levels_bytes >= 0 && sp.levels_bytes <= h.uncompressed && sp.levels_bytes <= h.compressed, "Parquet page levels overrun the page");
+    if (!sp.values_compressed)
+      SB_REQUIRE(h.compressed == h.uncompressed, "uncompressed Parquet page at byte %lld: %d stored bytes for %d", (long long)pos, h.compressed,
+                 h.uncompressed);
+    page(sp);
   }
-  *out_npages = np;
-  SB_API_END
 }
+
+// The sb_page descriptors and dictionary of one chunk, added span by span in page order (the last dictionary page counts), on
+// both paths, so a page is refused with the same message whether or not it was compressed.  body: where the decoded body starts
+// among the bytes the descriptors index; len4: its first 4 bytes (a V1 page's level length), nullptr when it is shorter;
+// values_head(pg): the first bytes of pg's values, where a DELTA_* header starts, and how many of them can be read.
+struct ChunkPages {
+  std::vector<sb_page> pages;
+  int64_t dict_offset = -1;
+  int32_t dict_count = 0;
+
+  template <class Head>
+  void add(const sb_page_span &sp, int32_t max_def_level, int64_t body, const uint8_t *len4, Head values_head) {
+    if (sp.page_type == 2) {
+      dict_offset = body;
+      dict_count = sp.num_values;
+      return;
+    }
+    sb_page pg;
+    memset(&pg, 0, sizeof(pg));
+    pg.encoding = sp.encoding;
+    pg.num_values = sp.num_values;
+    data_page_sections(pg, sp.page_type == 0, max_def_level, sp.levels_bytes, body, sp.uncompressed_bytes, len4);
+    if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED) {
+      const std::pair<const uint8_t *, int64_t> head = values_head(pg);
+      check_delta_header(head.first, head.second, pg.encoding, pg.num_values, (int)pages.size(), sp.body_offset - sp.header_bytes);
+    }
+    pages.push_back(pg);
+  }
+};
+}  // namespace
 
 static void require_codec(int32_t codec) {
   static const char *const names[] = {"UNCOMPRESSED", "SNAPPY", "GZIP", "LZO", "BROTLI", "LZ4", "ZSTD", "LZ4_RAW"};
   if (codec == SB_CODEC_UNCOMPRESSED || codec == SB_CODEC_SNAPPY) return;
   if (codec > 0 && codec < 8) fail(SB_ERR_UNSUPPORTED, "Parquet compression codec %s is not supported by the GPU scan (UNCOMPRESSED and SNAPPY are)", names[codec]);
   fail(SB_ERR_UNSUPPORTED, "Parquet compression codec %d is not supported by the GPU scan (UNCOMPRESSED and SNAPPY are)", codec);
+}
+
+// Host only (no device needed): the descriptors sb_scan_decode takes for one column chunk as it lies in a Parquet file.
+// max_def_level: 0 for a required column, 1 for an optional one.
+extern "C" int sb_parquet_chunk_pages(const uint8_t *chunk, int64_t nbytes, int32_t max_def_level, sb_page *out_pages, int32_t pages_cap,
+                                      int32_t *out_npages, int64_t *out_dict_offset, int32_t *out_dict_count) {
+  SB_API_BEGIN
+  SB_REQUIRE(chunk && out_pages && out_npages && out_dict_offset && out_dict_count && nbytes >= 0, "null argument");
+  ChunkPages cp;
+  walk_pages(chunk, nbytes, SB_CODEC_UNCOMPRESSED, max_def_level, true, pages_cap, false, [&](const sb_page_span &sp) {
+    cp.add(sp, max_def_level, sp.body_offset, sp.uncompressed_bytes >= 4 ? chunk + sp.body_offset : nullptr,
+           [&](const sb_page &pg) { return std::make_pair(chunk + pg.values_offset, pg.values_bytes); });
+  });
+  std::copy(cp.pages.begin(), cp.pages.end(), out_pages);
+  *out_npages = (int32_t)cp.pages.size();
+  *out_dict_offset = cp.dict_offset;
+  *out_dict_count = cp.dict_count;
+  SB_API_END
 }
 
 // Host only: the spans of a chunk whose pages may be compressed.  Unlike sb_parquet_chunk_pages it never looks inside a body:
@@ -1052,42 +1109,8 @@ extern "C" int sb_parquet_page_spans(const uint8_t *chunk, int64_t nbytes, int32
   SB_API_BEGIN
   SB_REQUIRE(chunk && out && out_n && nbytes >= 0, "null argument");
   require_codec(codec);
-  SB_REQUIRE(max_def_level == 0 || max_def_level == 1, "nested schemas are not supported (max definition level %d)", max_def_level);
   int32_t n = 0;
-  int64_t pos = 0;
-  while (pos < nbytes) {
-    Thrift t{chunk + pos, chunk + nbytes};
-    PageHeader h;
-    if (!read_page_header(t, h)) fail(SB_ERR_INVALID, "malformed Parquet page header at byte %lld of the column chunk", (long long)pos);
-    const int64_t body = t.p - chunk;
-    SB_REQUIRE(h.compressed >= 0 && h.uncompressed >= 0 && body + h.compressed <= nbytes, "Parquet page at byte %lld overruns the column chunk",
-               (long long)pos);
-    if (h.type == 0 || h.type == 2 || h.type == 3) {
-      SB_REQUIRE(n < cap, "more than %d pages in the column chunk", cap);
-      sb_page_span &sp = out[n++];
-      memset(&sp, 0, sizeof(sp));
-      sp.page_type = h.type;
-      sp.num_values = h.num_values;
-      sp.body_offset = body;
-      sp.header_bytes = (int32_t)(body - pos);
-      sp.compressed_bytes = h.compressed;
-      sp.uncompressed_bytes = h.uncompressed;
-      sp.values_compressed = codec != SB_CODEC_UNCOMPRESSED && !(h.is_v2 && !h.v2_compressed);
-      if (h.type == 2) {
-        SB_REQUIRE(h.encoding == 0 || h.encoding == 2, "dictionary page encoding %d is not PLAIN", h.encoding);
-        sp.encoding = SB_ENC_PLAIN;
-      } else {
-        sp.encoding = page_encoding(h.encoding);
-        check_data_page_header(h, max_def_level);
-        if (h.type == 3) sp.levels_bytes = h.def_len;
-      }
-      SB_REQUIRE(sp.levels_bytes >= 0 && sp.levels_bytes <= h.uncompressed && sp.levels_bytes <= h.compressed, "Parquet page levels overrun the page");
-      if (!sp.values_compressed)
-        SB_REQUIRE(h.compressed == h.uncompressed, "uncompressed Parquet page at byte %lld: %d stored bytes for %d", (long long)pos, h.compressed,
-                   h.uncompressed);
-    }   // INDEX_PAGE and unknown page types are skipped
-    pos = body + h.compressed;
-  }
+  walk_pages(chunk, nbytes, codec, max_def_level, false, cap, true, [&](const sb_page_span &sp) { out[n++] = sp; });
   *out_n = n;
   SB_API_END
 }
@@ -1099,6 +1122,11 @@ static int phys_width_of(int32_t physical) {
     case SB_PHYS_INT64: case SB_PHYS_DOUBLE: return 8;
   }
   fail(SB_ERR_UNSUPPORTED, "Parquet physical type %d is not supported by the GPU scan (BOOLEAN, INT32, INT64, FLOAT, DOUBLE are)", physical);
+}
+
+// [offset, offset + bytes) lies inside a chunk of chunk_bytes bytes (written so that no sum can overflow)
+static bool in_chunk(int64_t offset, int64_t bytes, int64_t chunk_bytes) {
+  return offset >= 0 && bytes >= 0 && offset <= chunk_bytes && bytes <= chunk_bytes - offset;
 }
 
 // host state of one sb_scan_decode call that the stream reads asynchronously (freed by a host function behind the kernels)
@@ -1214,18 +1242,51 @@ static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols
         SB_REQUIRE(ch.value_multiplier >= 0 && (ch.value_multiplier <= 1 || (ch.physical_type == SB_PHYS_INT64 && (ch.type == SB_TIMESTAMP || ch.type == SB_INT64))),
                    "column chunk %d: value multiplier %d applies to INT64 timestamp / long columns only", ci, ch.value_multiplier);
       }
+      // an all-NULL chunk has an empty dictionary page; an entry takes at least 4 bytes (a PLAIN byte array's length) or its
+      // physical width (one byte for BOOLEAN)
+      const bool has_dict = ch.dict_offset >= 0 && ch.dict_count >= 0;
+      SB_REQUIRE(!has_dict || in_chunk(ch.dict_offset, (int64_t)ch.dict_count * (is_str ? 4 : std::max(pw, 1)), ch.data_bytes),
+                 "column chunk %d: dictionary overruns the chunk", ci);
+      const uint8_t *dev = device_bytes(ch, temps);
       int64_t rows = 0;
-      bool nullable = false;
+      bool nullable = false, has_dba = false;
       for (int p = 0; p < ch.npages; p++) {
-        rows += ch.pages[p].num_values;
-        nullable |= ch.pages[p].def_bytes > 0;
+        const sb_page &pg = ch.pages[p];
+        const int32_t e = pg.encoding;
+        SB_REQUIRE(pg.num_values >= 0, "column chunk %d page %d has a negative value count (%d)", ci, p, pg.num_values);
+        SB_REQUIRE(in_chunk(pg.values_offset, pg.values_bytes, ch.data_bytes) && in_chunk(pg.def_offset, pg.def_bytes, ch.data_bytes),
+                   "column chunk %d page %d: offsets outside the chunk", ci, p);
+        SB_REQUIRE(e == SB_ENC_PLAIN || (e == SB_ENC_RLE_DICTIONARY && has_dict) ||
+                       (is_str ? e == SB_ENC_DELTA_LENGTH_BYTE_ARRAY || e == SB_ENC_DELTA_BYTE_ARRAY
+                               : (e == SB_ENC_RLE_BOOLEAN && pw == 0) ||
+                                     (e == SB_ENC_DELTA_BINARY_PACKED && (ch.physical_type == SB_PHYS_INT32 || ch.physical_type == SB_PHYS_INT64))),
+                   "column chunk %d page %d: encoding %d%s", ci, p, e,
+                   e == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : is_str ? " is not supported for BYTE_ARRAY columns" : " is not supported for this column");
+        PageTask pt;
+        pt.values = dev + pg.values_offset;
+        pt.values_bytes = pg.values_bytes;
+        pt.def = pg.def_bytes > 0 ? dev + pg.def_offset : nullptr;
+        pt.def_bytes = pg.def_bytes;
+        pt.row_start = rows;
+        pt.num_values = pg.num_values;
+        pt.encoding = e;
+        pt.col = ci;
+        pt.pad = 0;
+        if (!is_str) {
+          (e == SB_ENC_DELTA_BINARY_PACKED ? keep->delta_tasks : tasks).push_back(pt);
+        } else if (pg.num_values > 0) {
+          keep->str_pages.push_back(pt);
+          if (e == SB_ENC_DELTA_BYTE_ARRAY) keep->dba_pages.push_back(pt);
+        }
+        rows += pg.num_values;
+        nullable |= pg.def_bytes > 0;
+        has_dba |= e == SB_ENC_DELTA_BYTE_ARRAY;
       }
       if (nrows < 0) {
         nrows = rows;
         t = table_new(nrows);
       }
       SB_REQUIRE(rows == nrows, "column chunk %d has %lld rows, chunk 0 has %lld", ci, (long long)rows, (long long)nrows);
-      const uint8_t *dev = device_bytes(ch, temps);
       if (is_str) {
         Column col;
         col.type = SB_STRING;
@@ -1234,8 +1295,6 @@ static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols
         col.offsets = buffer_alloc((nrows + 1) * 4 + 16, st);
         if (nullable) col.validity = buffer_alloc(bitmap_alloc_bytes(nrows), st);
         t->cols.push_back(col);
-        bool has_dba = false;
-        for (int p = 0; p < ch.npages; p++) has_dba |= ch.pages[p].encoding == SB_ENC_DELTA_BYTE_ARRAY;
         StrColTask &sc = stasks[ci];
         memset(&sc, 0, sizeof(sc));
         sc.base = dev;
@@ -1250,38 +1309,12 @@ static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols
           sc.vpre = has_dba ? (int32_t *)scratch(nrows * 4 + 16) : nullptr;
         }
         ctasks[ci].valid_bytes = sc.valid_bytes;
-        const bool has_dict = ch.dict_offset >= 0 && ch.dict_count >= 0;
-        if (has_dict) {   // every PLAIN byte array takes at least its 4-byte length
-          SB_REQUIRE(ch.dict_offset + (int64_t)ch.dict_count * 4 <= ch.data_bytes, "column chunk %d: dictionary overruns the chunk", ci);
+        if (has_dict) {
           sc.dict_offset = ch.dict_offset;
           sc.dict_count = ch.dict_count;
           sc.dict_len = (int32_t *)scratch((int64_t)ch.dict_count * 4 + 16);
           sc.dict_src = (int64_t *)scratch((int64_t)ch.dict_count * 8 + 16);
           if (ch.dict_count > 0) keep->dict_cols.push_back(ci);
-        }
-        int64_t row = 0;
-        for (int p = 0; p < ch.npages; p++) {
-          const sb_page &pg = ch.pages[p];
-          SB_REQUIRE(pg.values_offset >= 0 && pg.values_bytes >= 0 && pg.values_offset + pg.values_bytes <= ch.data_bytes && pg.def_offset >= 0 &&
-                         pg.def_offset + pg.def_bytes <= ch.data_bytes,
-                     "column chunk %d page %d: offsets outside the chunk", ci, p);
-          SB_REQUIRE(pg.encoding == SB_ENC_PLAIN || (pg.encoding == SB_ENC_RLE_DICTIONARY && has_dict) || pg.encoding == SB_ENC_DELTA_LENGTH_BYTE_ARRAY ||
-                         pg.encoding == SB_ENC_DELTA_BYTE_ARRAY,
-                     "column chunk %d page %d: encoding %d%s", ci, p, pg.encoding,
-                     pg.encoding == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : " is not supported for BYTE_ARRAY columns");
-          PageTask pt;
-          pt.values = dev + pg.values_offset;
-          pt.values_bytes = pg.values_bytes;
-          pt.def = pg.def_bytes > 0 ? dev + pg.def_offset : nullptr;
-          pt.def_bytes = pg.def_bytes;
-          pt.row_start = row;
-          pt.num_values = pg.num_values;
-          pt.encoding = pg.encoding;
-          pt.col = ci;
-          pt.pad = 0;
-          if (pg.num_values > 0) keep->str_pages.push_back(pt);
-          if (pg.num_values > 0 && pg.encoding == SB_ENC_DELTA_BYTE_ARRAY) keep->dba_pages.push_back(pt);
-          row += pg.num_values;
         }
         keep->str_cols.push_back(ci);
         continue;
@@ -1299,38 +1332,11 @@ static sb_table *scan_decode_chunks(const sb_column_chunk *chunks, int32_t ncols
         ct.valid_bytes = vb->as<uint8_t>();
         ct.dense = dn->as<uint8_t>();
       }
-      ct.dict = nullptr;
-      ct.dict_count = 0;
-      if (ch.dict_offset >= 0 && ch.dict_count >= 0) {   // an all-NULL chunk has an empty dictionary page
-        SB_REQUIRE(ch.dict_offset + (int64_t)ch.dict_count * (pw ? pw : 1) <= ch.data_bytes, "column chunk %d: dictionary overruns the chunk", ci);
-        ct.dict = dev + ch.dict_offset;
-        ct.dict_count = ch.dict_count;
-      }
+      ct.dict = has_dict ? dev + ch.dict_offset : nullptr;
+      ct.dict_count = has_dict ? ch.dict_count : 0;
       ct.phys_width = pw;
       ct.out_width = ow;
       ct.mul = ch.value_multiplier;
-      int64_t row = 0;
-      for (int p = 0; p < ch.npages; p++) {
-        const sb_page &pg = ch.pages[p];
-        SB_REQUIRE(pg.values_offset >= 0 && pg.values_offset + pg.values_bytes <= ch.data_bytes && pg.def_offset + pg.def_bytes <= ch.data_bytes,
-                   "column chunk %d page %d: offsets outside the chunk", ci, p);
-        SB_REQUIRE(pg.encoding == SB_ENC_PLAIN || (pg.encoding == SB_ENC_RLE_DICTIONARY && ct.dict) || (pg.encoding == SB_ENC_RLE_BOOLEAN && pw == 0) ||
-                       (pg.encoding == SB_ENC_DELTA_BINARY_PACKED && (ch.physical_type == SB_PHYS_INT32 || ch.physical_type == SB_PHYS_INT64)),
-                   "column chunk %d page %d: encoding %d%s", ci, p, pg.encoding,
-                   pg.encoding == SB_ENC_RLE_DICTIONARY ? " without a dictionary page" : " is not supported for this column");
-        PageTask pt;
-        pt.values = dev + pg.values_offset;
-        pt.values_bytes = pg.values_bytes;
-        pt.def = pg.def_bytes > 0 ? dev + pg.def_offset : nullptr;
-        pt.def_bytes = pg.def_bytes;
-        pt.row_start = row;
-        pt.num_values = pg.num_values;
-        pt.encoding = pg.encoding;
-        pt.col = ci;
-        pt.pad = 0;
-        (pg.encoding == SB_ENC_DELTA_BINARY_PACKED ? keep->delta_tasks : tasks).push_back(pt);
-        row += pg.num_values;
-      }
     }
     std::vector<PageTask> &dtasks = keep->delta_tasks;
     const bool queued = nrows > 0 && (!tasks.empty() || !dtasks.empty());
@@ -1415,9 +1421,10 @@ extern "C" int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int3
     int64_t off = 0;
     for (int p = 0; p < ch.npages; p++) {
       const sb_page_span &x = ch.spans[p];
-      SB_REQUIRE(x.body_offset >= 0 && x.compressed_bytes >= 0 && x.uncompressed_bytes >= 0 && x.body_offset + x.compressed_bytes <= ch.data_bytes &&
-                     x.levels_bytes >= 0 && x.levels_bytes <= x.compressed_bytes && x.levels_bytes <= x.uncompressed_bytes,
+      SB_REQUIRE(in_chunk(x.body_offset, x.compressed_bytes, ch.data_bytes) && x.uncompressed_bytes >= 0 && x.levels_bytes >= 0 &&
+                     x.levels_bytes <= x.compressed_bytes && x.levels_bytes <= x.uncompressed_bytes,
                  "column chunk %d page %d: span outside the chunk", ci, p);
+      SB_REQUIRE(x.num_values >= 0, "column chunk %d page %d has a negative value count (%d)", ci, p, x.num_values);
       SB_REQUIRE(x.values_compressed ? ch.codec == SB_CODEC_SNAPPY : x.compressed_bytes == x.uncompressed_bytes,
                  "column chunk %d page %d: %s page of %d stored bytes for %d", ci, p, x.values_compressed ? "compressed" : "uncompressed",
                  x.compressed_bytes, x.uncompressed_bytes);
@@ -1472,11 +1479,21 @@ extern "C" int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int3
     SB_CUDA(cudaStreamSynchronize(st));
   }
   raw.clear();
-  // the page checks of sb_parquet_chunk_pages, on the decoded pages
-  std::vector<std::vector<sb_page>> pages(ncols);
+  // the descriptors sb_parquet_chunk_pages builds, over the decoded pages
+  std::vector<ChunkPages> pages(ncols);
   std::vector<sb_column_chunk> dec(ncols);
   for (int ci = 0; ci < ncols; ci++) {
     const sb_compressed_chunk &ch = chunks[ci];
+    for (int p = 0; p < ch.npages; p++) {
+      const sb_page_span &x = ch.spans[p];
+      const PageRecord &r = recs[slot_base[ci] + p];
+      if (r.status != SNAPPY_OK)
+        fail(SB_ERR_INVALID, "column chunk %d page %d (byte %lld of the column chunk): malformed Snappy stream: %s", ci, p,
+             (long long)(x.body_offset - x.header_bytes), snappy_status_text(r.status));
+      pages[ci].add(x, ch.max_def_level, img_off[ci][p], r.body_short ? nullptr : (const uint8_t *)&r.def_len, [&](const sb_page &pg) {
+        return std::make_pair((const uint8_t *)r.head, std::min<int64_t>(r.head_bytes, pg.values_bytes));
+      });
+    }
     sb_column_chunk &d = dec[ci];
     memset(&d, 0, sizeof(d));
     d.type = ch.type;
@@ -1485,32 +1502,10 @@ extern "C" int sb_scan_decode_compressed(const sb_compressed_chunk *chunks, int3
     d.value_multiplier = ch.value_multiplier;
     d.data = images[ci]->as<uint8_t>();   // the image (device); scan_decode_chunks reads it through device_bytes only
     d.data_bytes = img_bytes[ci];
-    d.dict_offset = -1;
-    for (int p = 0; p < ch.npages; p++) {
-      const sb_page_span &x = ch.spans[p];
-      const PageRecord &r = recs[slot_base[ci] + p];
-      const int64_t header_at = x.body_offset - x.header_bytes;
-      if (r.status != SNAPPY_OK)
-        fail(SB_ERR_INVALID, "column chunk %d page %d (byte %lld of the column chunk): malformed Snappy stream: %s", ci, p, (long long)header_at,
-             snappy_status_text(r.status));
-      if (x.page_type == 2) {
-        d.dict_offset = img_off[ci][p];
-        d.dict_count = x.num_values;
-        continue;
-      }
-      sb_page pg;
-      memset(&pg, 0, sizeof(pg));
-      pg.encoding = x.encoding;
-      pg.num_values = x.num_values;
-      const int dp = (int)pages[ci].size();
-      data_page_sections(pg, x.page_type == 0, ch.max_def_level, x.levels_bytes, img_off[ci][p], x.uncompressed_bytes,
-                         r.body_short ? nullptr : (const uint8_t *)&r.def_len);
-      if (pg.encoding >= SB_ENC_DELTA_BINARY_PACKED)
-        check_delta_header(r.head, std::min<int64_t>(r.head_bytes, pg.values_bytes), pg.encoding, x.num_values, dp, header_at);
-      pages[ci].push_back(pg);
-    }
-    d.pages = pages[ci].data();
-    d.npages = (int32_t)pages[ci].size();
+    d.pages = pages[ci].pages.data();
+    d.npages = (int32_t)pages[ci].pages.size();
+    d.dict_offset = pages[ci].dict_offset;
+    d.dict_count = pages[ci].dict_count;
   }
   *out = scan_decode_chunks(dec.data(), ncols, st, [&](const sb_column_chunk &ch, std::vector<std::unique_ptr<Scratch>> &) { return ch.data; });
   SB_API_END
