@@ -110,7 +110,7 @@ constexpr int REMOTE_MAX_BUCKETS = 16;   // destinations of the fused exchange s
 // (low digit, then high digit -- "LSB radix partition").
 //
 // This first kernel is the load/store version: it is what runs when a source column is not 16-byte aligned (the copy engine
-// needs that) or with SB_REGROUP_PATH=ldst; the default is regroup_tma_kernel further down, which shares phases A-D.
+// needs that) or with sb_config_set("regroup_ldst", 1); the default is regroup_tma_kernel further down, which shares phases A-D.
 // A block owns a chunk of rows (one histogram column) and walks it in tiles of RGL_TILE rows.  Per tile:
 //   A  every warp owns a contiguous 1/16 of the tile and walks it 32 rows at a time: same-bucket rows are ranked with
 //      __match_any_sync + popcount on top of a per-warp shared-memory counter  -> (bucket, rank inside the warp's segment);
@@ -679,7 +679,8 @@ static void regroup_pass(const int32_t *bucket_dev, uint32_t *hist_dev, int32_t 
     }
     if (rc.ncols > 0 || (first && perm_out)) {
       // the copy engine wants 16-byte aligned sources; anything else (a caller-provided, oddly offset device buffer) takes the
-      // load/store kernel (sb_config_set("regroup_ldst", 1) forces it: the parity tests run both).
+      // load/store kernel.  sb_config_set("regroup_ldst", 1) forces it; the shuffle tests of tests/test_gpu_row_movement.py run
+      // with both settings, and a source borrowed one element past an aligned allocation takes it whatever the setting.
       const bool force_ldst = config().regroup_ldst != 0;
       bool aligned = ((uintptr_t)bucket_dev & 15) == 0;
       for (int k = 0; k < rc.ncols; k++) aligned = aligned && ((uintptr_t)rc.src[k] & 15) == 0;

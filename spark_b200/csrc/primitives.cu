@@ -128,6 +128,31 @@ __device__ __forceinline__ void gather_rows(const void *__restrict__ src, void *
   for (int k = 0; k < GATHER_ITEMS; k++)
     if (i0 + k * 256 < nout) ((T *)dst)[i0 + k * 256] = v[k];
 }
+template <bool ALIGNED16>
+__device__ __forceinline__ void gather_rows16(const void *__restrict__ src, void *__restrict__ dst, const int64_t (&j)[GATHER_ITEMS], int64_t i0,
+                                              int64_t nout) {
+#pragma unroll
+  for (int h = 0; h < 2; h++) {   // two halves: 16-byte values would double the register footprint
+    uint4 v[GATHER_ITEMS / 2];
+#pragma unroll
+    for (int k = 0; k < GATHER_ITEMS / 2; k++) {
+      const int64_t jj = j[h * (GATHER_ITEMS / 2) + k];
+      if (jj < 0) {
+        v[k] = make_uint4(0, 0, 0, 0);
+      } else if (ALIGNED16) {
+        v[k] = __ldg((const uint4 *)src + jj);
+      } else {
+        const uint2 lo = __ldg((const uint2 *)src + 2 * jj), hi = __ldg((const uint2 *)src + 2 * jj + 1);
+        v[k] = make_uint4(lo.x, lo.y, hi.x, hi.y);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < GATHER_ITEMS / 2; k++) {
+      const int64_t i = i0 + (h * (GATHER_ITEMS / 2) + k) * 256;
+      if (i < nout) ((uint4 *)dst)[i] = v[k];
+    }
+  }
+}
 __global__ void __launch_bounds__(256) gather_fixed_kernel(GatherArgs a, const int64_t *__restrict__ idx, int64_t nout) {
   const int64_t i0 = (int64_t)blockIdx.x * (256 * GATHER_ITEMS) + threadIdx.x;
   int64_t j[GATHER_ITEMS];
@@ -139,23 +164,12 @@ __global__ void __launch_bounds__(256) gather_fixed_kernel(GatherArgs a, const i
       case 1: gather_rows<uint8_t>(a.src[c], a.dst[c], j, i0, nout); break;
       case 2: gather_rows<uint16_t>(a.src[c], a.dst[c], j, i0, nout); break;
       case 4: gather_rows<uint32_t>(a.src[c], a.dst[c], j, i0, nout); break;
-      case 16: {
-#pragma unroll
-        for (int h = 0; h < 2; h++) {   // two halves: 16-byte values would double the register footprint
-          uint4 v[GATHER_ITEMS / 2];
-#pragma unroll
-          for (int k = 0; k < GATHER_ITEMS / 2; k++) {
-            const int64_t jj = j[h * (GATHER_ITEMS / 2) + k];
-            v[k] = jj >= 0 ? __ldg((const uint4 *)a.src[c] + jj) : make_uint4(0, 0, 0, 0);
-          }
-#pragma unroll
-          for (int k = 0; k < GATHER_ITEMS / 2; k++) {
-            const int64_t i = i0 + (h * (GATHER_ITEMS / 2) + k) * 256;
-            if (i < nout) ((uint4 *)a.dst[c])[i] = v[k];
-          }
-        }
+      case 16:
+        // a 16-byte load needs a 16-byte aligned source; a decimal128 column borrowed from device memory may be only 8-byte
+        // aligned (test_gpu_row_movement.py::test_shuffle_misaligned_source faulted on it), and then takes two 8-byte loads
+        if (((uintptr_t)a.src[c] & 15) == 0) gather_rows16<true>(a.src[c], a.dst[c], j, i0, nout);
+        else gather_rows16<false>(a.src[c], a.dst[c], j, i0, nout);
         break;
-      }
       default: gather_rows<uint64_t>(a.src[c], a.dst[c], j, i0, nout); break;
     }
     if (a.dst_valid[c]) {

@@ -99,7 +99,10 @@ class AttributeReference(Expression):
 
     def vtype(self, schema):
         t = schema.types[schema.index(self.name)]
-        if t == capi.SB_STRING:
+        # strings and decimal(p > 18) have no value class: they are only moved as bare references (the native side refuses them
+        # in arithmetic or comparisons).  Filter and expand over a decimal(38, s) column used to stop here with a KeyError
+        # (caught by test_gpu_row_movement.py::test_filter / test_expand).
+        if t in (capi.SB_STRING, capi.SB_DECIMAL128):
             return 0
         return _VT_OF_SB[t]
 
