@@ -382,6 +382,16 @@ int sb_round_robin_partition(const sb_table *in, int32_t start, int32_t num_part
 #define SB_AGG_COUNT_STAR 4
 #define SB_AGG_MIN 5
 #define SB_AGG_MAX 6
+/* central moments (CentralMomentAgg.scala:49-290): the input is read as DOUBLE (integer and float inputs are converted as
+ * Cast(_, DoubleType) does; decimal, string, boolean, date and timestamp inputs are SB_ERR_UNSUPPORTED); NULL inputs are skipped */
+#define SB_AGG_VAR_POP 7      /* m2 / n; NULL for n == 0 */
+#define SB_AGG_VAR_SAMP 8     /* m2 / (n - 1); NULL for n == 0; for n == 1 NULL, or NaN with SB_AGG_FLAG_NAN_ON_DIVIDE_BY_ZERO */
+#define SB_AGG_STDDEV_POP 9   /* sqrt(m2 / n) */
+#define SB_AGG_STDDEV_SAMP 10 /* sqrt(m2 / (n - 1)), n == 1 as for VAR_SAMP */
+
+/* sb_agg_spec.flags */
+#define SB_AGG_FLAG_NAN_ON_DIVIDE_BY_ZERO 1   /* _SAMP of one row gives NaN, not NULL (nullOnDivideByZero = false, i.e.
+                                                 spark.sql.legacy.statisticalAggregate); 0 is Spark's default */
 
 #define SB_AGG_MODE_PARTIAL 1   /* input rows -> keys ++ buffers  (AggUtils.scala:131-208) */
 #define SB_AGG_MODE_FINAL 2     /* keys ++ buffers -> keys ++ results */
@@ -390,7 +400,7 @@ int sb_round_robin_partition(const sb_table *in, int32_t start, int32_t num_part
 
 typedef struct sb_agg_spec {
   int32_t func;        /* SB_AGG_* */
-  int32_t pad;
+  int32_t flags;       /* SB_AGG_FLAG_* (0 for every function but VAR_SAMP / STDDEV_SAMP) */
   sb_expr input;       /* Partial/Complete: value expression (ignored for COUNT_STAR).
                           Final: ignored -- buffers are read positionally after the keys. */
 } sb_agg_spec;
@@ -408,7 +418,9 @@ typedef struct sb_agg_plan {
 } sb_agg_plan;
 
 /* Output: key columns, then per aggregate either its buffer columns (Partial: sum -> [sum];
- * avg -> [sum f64, count i64]; count -> [count]; min/max -> [value]) or its result column. */
+ * avg -> [sum f64, count i64]; count -> [count]; min/max -> [value]; var_* / stddev_* -> [n f64, avg f64, m2 f64], Spark's
+ * CentralMomentAgg buffer, (0.0, 0.0, 0.0) for a group without non-NULL input) or its result column (f64 for the moments).
+ * Final / PartialMerge read the same buffer columns positionally after the keys. */
 int sb_hash_aggregate(const sb_table *in, const sb_agg_plan *plan, sb_stream *s, sb_table **out);
 /* build check without a device: compiles the run-time specialisation of a plan given as its raw PlanMeta int32 words
  * (sb_agg_plan_meta_words() of them; layout = csrc/agg_kernels.cuh) and returns the compiler's verdict */

@@ -81,7 +81,8 @@ JNIEXPORT jlong JNICALL Java_org_apache_spark_sql_b200_Native_hashAggregate(
   jlong *in = (*env)->GetLongArrayElements(env, inputExprs, NULL);
   sb_agg_spec *specs = (sb_agg_spec *)calloc((size_t)(na ? na : 1), sizeof(sb_agg_spec));
   for (jsize i = 0; i < na; i++) {
-    specs[i].func = f[i];
+    specs[i].func = f[i] & 0xFFFF;    /* funcs[i] = SB_AGG_* | sb_agg_spec.flags << 16 */
+    specs[i].flags = f[i] >> 16;
     if (in[i]) specs[i].input = *(const sb_expr *)(intptr_t)in[i];
   }
   sb_agg_plan plan = {mode, nk, (const int32_t *)k, na, 0, specs, (const sb_expr *)(intptr_t)filterExpr, expectedGroups};
@@ -400,7 +401,8 @@ NATIVE(jlong, aggCreate)(JNIEnv *env, jclass c, jint mode, jintArray keyCols, ji
   jlong *in = (*env)->GetLongArrayElements(env, inputExprs, NULL);
   sb_agg_spec *specs = (sb_agg_spec *)calloc((size_t)(na ? na : 1), sizeof(sb_agg_spec));
   for (jsize i = 0; i < na; i++) {
-    specs[i].func = f[i];
+    specs[i].func = f[i] & 0xFFFF;    /* funcs[i] = SB_AGG_* | sb_agg_spec.flags << 16 */
+    specs[i].flags = f[i] >> 16;
     if (in[i]) specs[i].input = *(const sb_expr *)(intptr_t)in[i];
   }
   sb_agg_plan plan = {mode, nk, (const int32_t *)k, na, 0, specs, (const sb_expr *)(intptr_t)filterExpr, expectedGroups};

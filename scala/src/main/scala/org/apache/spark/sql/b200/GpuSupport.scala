@@ -35,6 +35,13 @@ object GpuSupport {
     case d: DecimalType => d.precision <= 18 && c.isInstanceOf[AttributeReference]
     case _ => true
   }
+  /** central moments read their input as DOUBLE: a double expression, or the analyzer's Cast to DOUBLE of an integer or float one
+   *  (decimal, boolean, string, date and timestamp inputs are not taken) */
+  private def momentInputOk(c: Expression): Boolean = exprOk(c) && (c match {
+    case cast: Cast if cast.dataType == DoubleType =>
+      cast.child.dataType match { case ByteType | ShortType | IntegerType | LongType | FloatType | DoubleType => true; case _ => false }
+    case _ => c.dataType == DoubleType
+  })
   /** grouping / join / sort keys: fixed-width types, and strings (order-preserving dictionary codes inside the library) */
   private def keyOk(dt: DataType): Boolean = fixedWidth(dt) || dt == StringType
 
@@ -52,7 +59,11 @@ object GpuSupport {
           case Count(cs) => cs.length <= 1 && cs.forall(exprOk)
           case Min(c) => fixedWidth(c.dataType) && exprOk(c)
           case Max(c) => fixedWidth(c.dataType) && exprOk(c)
-          case _ => false
+          case VariancePop(c, _) => momentInputOk(c)
+          case VarianceSamp(c, _) => momentInputOk(c)
+          case StddevPop(c, _) => momentInputOk(c)
+          case StddevSamp(c, _) => momentInputOk(c)
+          case _ => false      // Skewness, Kurtosis, covariance / correlation and the Pandas forms stay on the CPU
         })
       }
   def supports(s: SortExec): Boolean = outputOk(s.child) &&
@@ -208,6 +219,11 @@ object GpuSupport {
       case Count(cs) => if (cs.isEmpty || cs.forall(!_.nullable)) 4 else 3
       case _: Min => 5
       case _: Max => 6
+      // SB_AGG_VAR_POP .. SB_AGG_STDDEV_SAMP; bits 16.. carry sb_agg_spec.flags (SB_AGG_FLAG_NAN_ON_DIVIDE_BY_ZERO = 1)
+      case VariancePop(_, _) => 7
+      case VarianceSamp(_, nullOnDivideByZero) => 8 | (if (nullOnDivideByZero) 0 else 1 << 16)
+      case StddevPop(_, _) => 9
+      case StddevSamp(_, nullOnDivideByZero) => 10 | (if (nullOnDivideByZero) 0 else 1 << 16)
     }).toArray
     Lowerable(keyCols, funcs, inputs.map(_.map(e => ExprCompiler.compile(e, in))).toArray, condition.map(ExprCompiler.compile(_, in)))
   }

@@ -25,7 +25,8 @@ SB_OP = dict(COL=1, LIT_I64=2, LIT_F64=3, LIT_NULL=4, ADD=10, SUB=11, MUL=12, DI
              SF_RPAD=79)
 SB_SF_MAX_RANGES = 16
 SB_VT_BOOL, SB_VT_I32, SB_VT_I64, SB_VT_F64 = 1, 2, 3, 4
-SB_AGG = dict(sum=1, avg=2, count=3, count_star=4, min=5, max=6)
+SB_AGG = dict(sum=1, avg=2, count=3, count_star=4, min=5, max=6, var_pop=7, var_samp=8, stddev_pop=9, stddev_samp=10)
+SB_AGG_FLAG_NAN_ON_DIVIDE_BY_ZERO = 1
 SB_AGG_MODE = dict(partial=1, final=2, complete=3, partial_merge=4)
 SB_JOIN = dict(inner=0, left_outer=1, left_semi=2, left_anti=3, full_outer=4, build_outer=5, existence=6, left_anti_null_aware=7)
 SB_UNIQUE_ID_BYTES = 128
@@ -88,7 +89,7 @@ class sb_expr(C.Structure):
 
 
 class sb_agg_spec(C.Structure):
-    _fields_ = [("func", C.c_int32), ("pad", C.c_int32), ("input", sb_expr)]
+    _fields_ = [("func", C.c_int32), ("flags", C.c_int32), ("input", sb_expr)]
 
 
 class sb_agg_plan(C.Structure):

@@ -1029,10 +1029,70 @@ __device__ __forceinline__ int64_t table_slot_wide(const AggArgs &a, const uint6
   return -1;
 }
 
+// keep / packed multi-word group key of the thread's rows (the wide-key counterpart of tile_keys)
+template <int NW, int ITEMS>
+__device__ __forceinline__ void tile_keys_wide(const AggArgs &a, const TileCtx &t, bool (&keep)[ITEMS], uint64_t (&key)[ITEMS][NW]) {
+  using P = DynPlan;
+  const PlanMeta &m = a.meta;
+#pragma unroll
+  for (int k = 0; k < ITEMS; k++) {
+    keep[k] = t.row0 + (int64_t)k * AGG_THREADS <= t.last;
+#pragma unroll
+    for (int i = 0; i < NW; i++) key[k][i] = 0;
+  }
+  if (m.has_mask) {
+    int64_t x[ITEMS];
+    load_batch_as_i64<ITEMS, false, uint8_t>(a.col[m.mask_col].data, t, x);
+#pragma unroll
+    for (int k = 0; k < ITEMS; k++) keep[k] = keep[k] && x[k] != 0;
+  }
+  apply_filter_terms<P, ITEMS, false>(a, t, keep);
+  for (int i = 0; i < m.nkeys; i++) {
+    const int kt = m.key_type[i], bits = m.key_bits[i], shift = m.key_shift[i];
+    const KeyExtra ke = a.key_extra[i];
+    int64_t x[ITEMS];
+    bool valid[ITEMS];
+    if (kt == SB_FLOAT64) load_batch_as_i64<ITEMS, false, int64_t>(a.col[m.key_col[i]].data, t, x);
+    else load_i64_batch<ITEMS, false>(a.col[m.key_col[i]].data, kt, t, x);
+    if (m.key_valid[i]) load_valid_batch<ITEMS, false>(a.col[m.key_col[i]].valid, t, valid);
+#pragma unroll
+    for (int k = 0; k < ITEMS; k++) {
+      if (m.key_valid[i] && !valid[k]) {
+        const uint64_t nb = 1ull << m.key_nshift[i];
+#pragma unroll
+        for (int wi = 0; wi < NW; wi++)
+          if (wi == ke.null_word) key[k][wi] |= nb;
+        continue;
+      }
+      uint64_t v;
+      if (kt == SB_FLOAT32) {
+        float f = __int_as_float((int32_t)x[k]);
+        v = f == 0.0f ? 0u : (uint32_t)float_bits_canonical(f);
+      } else if (kt == SB_FLOAT64) {
+        double d = __longlong_as_double(x[k]);
+        v = d == 0.0 ? 0ull : (uint64_t)double_bits_canonical(d);
+      } else {
+        v = (uint64_t)x[k];
+        if (bits < 64) v &= (1ull << bits) - 1;
+      }
+      if (bits == 64) {   // 63 payload bits per word: bit 63 lives elsewhere
+        const uint64_t hi = (v >> 63) << ke.hi_shift;
+#pragma unroll
+        for (int wi = 0; wi < NW; wi++)
+          if (wi == ke.hi_word) key[k][wi] |= hi;
+        v &= 0x7FFFFFFFFFFFFFFFull;
+      }
+      v <<= shift;
+#pragma unroll
+      for (int wi = 0; wi < NW; wi++)
+        if (wi == ke.word) key[k][wi] |= v;
+    }
+  }
+}
+
 template <int NW, int ITEMS>
 __global__ void __launch_bounds__(AGG_THREADS) agg_update_wide_kernel(const __grid_constant__ AggArgs a) {
   using P = DynPlan;
-  const PlanMeta &m = a.meta;
   const int tid = threadIdx.x;
   constexpr int64_t TILE = (int64_t)AGG_THREADS * ITEMS;
   const int64_t stride = a.cap + 2;
@@ -1041,60 +1101,7 @@ __global__ void __launch_bounds__(AGG_THREADS) agg_update_wide_kernel(const __gr
     TileCtx t{base + tid, a.n - 1};
     bool keep[ITEMS];
     uint64_t key[ITEMS][NW];
-#pragma unroll
-    for (int k = 0; k < ITEMS; k++) {
-      keep[k] = t.row0 + (int64_t)k * AGG_THREADS <= t.last;
-#pragma unroll
-      for (int i = 0; i < NW; i++) key[k][i] = 0;
-    }
-    if (m.has_mask) {
-      int64_t x[ITEMS];
-      load_batch_as_i64<ITEMS, false, uint8_t>(a.col[m.mask_col].data, t, x);
-#pragma unroll
-      for (int k = 0; k < ITEMS; k++) keep[k] = keep[k] && x[k] != 0;
-    }
-    apply_filter_terms<P, ITEMS, false>(a, t, keep);
-    for (int i = 0; i < m.nkeys; i++) {
-      const int kt = m.key_type[i], bits = m.key_bits[i], shift = m.key_shift[i];
-      const KeyExtra ke = a.key_extra[i];
-      int64_t x[ITEMS];
-      bool valid[ITEMS];
-      if (kt == SB_FLOAT64) load_batch_as_i64<ITEMS, false, int64_t>(a.col[m.key_col[i]].data, t, x);
-      else load_i64_batch<ITEMS, false>(a.col[m.key_col[i]].data, kt, t, x);
-      if (m.key_valid[i]) load_valid_batch<ITEMS, false>(a.col[m.key_col[i]].valid, t, valid);
-#pragma unroll
-      for (int k = 0; k < ITEMS; k++) {
-        if (m.key_valid[i] && !valid[k]) {
-          const uint64_t nb = 1ull << m.key_nshift[i];
-#pragma unroll
-          for (int wi = 0; wi < NW; wi++)
-            if (wi == ke.null_word) key[k][wi] |= nb;
-          continue;
-        }
-        uint64_t v;
-        if (kt == SB_FLOAT32) {
-          float f = __int_as_float((int32_t)x[k]);
-          v = f == 0.0f ? 0u : (uint32_t)float_bits_canonical(f);
-        } else if (kt == SB_FLOAT64) {
-          double d = __longlong_as_double(x[k]);
-          v = d == 0.0 ? 0ull : (uint64_t)double_bits_canonical(d);
-        } else {
-          v = (uint64_t)x[k];
-          if (bits < 64) v &= (1ull << bits) - 1;
-        }
-        if (bits == 64) {   // 63 payload bits per word: bit 63 lives elsewhere
-          const uint64_t hi = (v >> 63) << ke.hi_shift;
-#pragma unroll
-          for (int wi = 0; wi < NW; wi++)
-            if (wi == ke.hi_word) key[k][wi] |= hi;
-          v &= 0x7FFFFFFFFFFFFFFFull;
-        }
-        v <<= shift;
-#pragma unroll
-        for (int wi = 0; wi < NW; wi++)
-          if (wi == ke.word) key[k][wi] |= v;
-      }
-    }
+    tile_keys_wide<NW, ITEMS>(a, t, keep, key);
     int64_t dst[ITEMS];
     int doff[ITEMS];
 #pragma unroll

@@ -38,6 +38,7 @@
 #include "rtc.cuh"
 #include "strings.cuh"
 #include "decimal.cuh"
+#include "moments.cuh"
 
 namespace sb {
 
@@ -515,6 +516,7 @@ struct AggBuilder {
 
 static bool is_float_type(int32_t t) { return t == SB_FLOAT32 || t == SB_FLOAT64; }
 
+constexpr int OUT_MOMENT = -1;   // OutPlan::op of a column moments_run writes (csrc/moments.cu)
 struct OutPlan {   // one output column
   int op, out_type, slot, slot2, xform;
   bool nullable;
@@ -551,6 +553,9 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
     return m.ncols++;
   };
   std::vector<OutPlan> outs;
+  std::vector<MomentInput> mom_in;
+  std::vector<MomentOut> mom_out;
+  std::vector<int> mom_first_out;   // index in `outs` of each moment aggregate's first column
   HostRef mask_ref, term_refs[AGG_MAX_TERMS], key_refs[AGG_MAX_KEYS];
   void *mask_ptr = nullptr;
 
@@ -745,6 +750,76 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
         c.kind = K_ADD_I64; c.is_one = 1; c.xform = X_NONE;
         int seen = b.add_slot(c);
         outs.push_back({E_MINMAX, src_type, main, seen, s.xform, true, src_type == SB_DECIMAL64 ? src_scale : 0});
+        break;
+      }
+      case SB_AGG_VAR_POP: case SB_AGG_VAR_SAMP: case SB_AGG_STDDEV_POP: case SB_AGG_STDDEV_SAMP: {
+        // CentralMomentAgg: pass 1 (these slots) gives each group's count, mean and range, pass 2 (csrc/moments.cu) the deviations
+        SB_REQUIRE((sp.flags & ~SB_AGG_FLAG_NAN_ON_DIVIDE_BY_ZERO) == 0, "unknown aggregate flags %d", sp.flags);
+        MomentInput mi;
+        memset(&mi, 0, sizeof(mi));
+        auto col_slot = [](const Column &c, const uint8_t *valid, int kind, int xform) {
+          HostSlot s;
+          s.nf = 1;
+          s.f[0].data = c.d(); s.f[0].valid = valid; s.f[0].type = c.type; s.f[0].mode = F_COL;
+          s.kind = kind; s.xform = xform;
+          return s;
+        };
+        if (final_mode) {   // buffers (n, avg, m2): SUM(n), SUM(n * avg), MIN / MAX(avg) over the non-empty partials
+          SB_REQUIRE(next_buf_col + 2 < (int)in->cols.size(), "Final aggregate: a variance / stddev buffer is (n, avg, m2) at column %d", next_buf_col);
+          const Column &nc = in->cols[next_buf_col], &ac = in->cols[next_buf_col + 1], &mc = in->cols[next_buf_col + 2];
+          SB_REQUIRE(nc.type == SB_FLOAT64 && ac.type == SB_FLOAT64 && mc.type == SB_FLOAT64, "variance / stddev buffers (n, avg, m2) must be float64");
+          next_buf_col += 3;
+          Column n_m, avg_m;
+          moments_mask_buffers(nc, ac, mc, n_m, avg_m, st);
+          b.temps.push_back(n_m);
+          b.temps.push_back(avg_m);
+          mi.x = avg_m.d(); mi.xv = avg_m.v(); mi.xtype = SB_FLOAT64;
+          mi.n = (const double *)n_m.d(); mi.m2 = (const double *)mc.d();
+          mi.slot_cnt = b.add_slot(col_slot(n_m, nullptr, K_ADD_F64, X_NONE));
+          HostSlot prod = col_slot(n_m, nullptr, K_ADD_F64, X_NONE);
+          prod.nf = 2;
+          prod.f[1] = col_slot(avg_m, avg_m.v(), K_ADD_F64, X_NONE).f[0];
+          mi.slot_sum = b.add_slot(prod);
+          mi.slot_min = b.add_slot(col_slot(avg_m, avg_m.v(), K_MIN_U64, X_DOUBLE));
+          mi.slot_max = b.add_slot(col_slot(avg_m, avg_m.v(), K_MAX_U64, X_DOUBLE));
+        } else {            // the input as DOUBLE: COUNT, SUM, MIN, MAX of x
+          int c;
+          Column src;
+          const sb_expr &e = sp.input;
+          if (expr_is_column(e, &c) || (e.n == 2 && e.nodes[0].op == SB_OP_COL && e.nodes[1].op == SB_OP_CAST_F64 && (c = e.nodes[0].arg, true))) {
+            SB_REQUIRE(c >= 0 && c < (int)in->cols.size(), "aggregate input column %d out of range", c);
+            src = in->cols[c];   // a numeric column is read as double in the kernels: what Cast(_, DoubleType) does
+          } else {
+            expr_validate(in, e);
+            src = eval_projection(in, e, nullptr, in->nrows, st);
+            b.temps.push_back(src);
+          }
+          if (src.type < SB_INT8 || src.type > SB_FLOAT64) fail(SB_ERR_UNSUPPORTED, "variance / stddev of a column of type %d is not supported", src.type);
+          const uint8_t *valid = nulls_of(src);
+          mi.x = src.d(); mi.xv = valid; mi.xtype = src.type;
+          HostSlot cnt = col_slot(src, valid, K_ADD_I64, X_NONE);
+          cnt.is_one = 1;
+          mi.slot_cnt = b.add_slot(cnt);
+          mi.slot_sum = b.add_slot(col_slot(src, valid, K_ADD_F64, X_NONE));
+          mi.slot_min = b.add_slot(col_slot(src, valid, K_MIN_U64, X_DOUBLE));
+          mi.slot_max = b.add_slot(col_slot(src, valid, K_MAX_U64, X_DOUBLE));
+        }
+        MomentOut mo;
+        memset(&mo, 0, sizeof(mo));
+        mo.input = -1;
+        for (size_t j = 0; j < mom_in.size(); j++)   // var(x) and stddev(x) share their passes
+          if (mom_in[j].slot_cnt == mi.slot_cnt && mom_in[j].slot_sum == mi.slot_sum && mom_in[j].slot_min == mi.slot_min &&
+              mom_in[j].slot_max == mi.slot_max)
+            mo.input = (int32_t)j;
+        if (mo.input < 0) {
+          mo.input = (int32_t)mom_in.size();
+          mom_in.push_back(mi);
+        }
+        mo.func = sp.func;
+        mo.flags = sp.flags;
+        mom_out.push_back(mo);
+        mom_first_out.push_back((int)outs.size());
+        for (int k = 0; k < (emit_buffers ? 3 : 1); k++) outs.push_back({OUT_MOMENT, SB_FLOAT64, -1, -1, X_NONE, !emit_buffers});
         break;
       }
       default: fail(SB_ERR_INVALID, "unknown aggregate function %d", sp.func);
@@ -961,23 +1036,31 @@ static void hash_aggregate_fixed(const sb_table *in, const sb_agg_plan *plan, cu
       e.key[k].hi_word = a.key_extra[k].hi_word;
       e.key[k].hi_shift = a.key_extra[k].hi_shift;
     }
-    SB_REQUIRE(outs.size() <= 2 * AGG_MAX_SLOTS, "too many aggregate output columns");
-    e.ncols = (int)outs.size();
+    e.ncols = 0;
     for (size_t i = 0; i < outs.size(); i++) {
       Column c = column_alloc(outs[i].out_type, outs[i].scale, ngroups, outs[i].nullable, st);
       t->cols.push_back(c);
-      e.col[i].out = c.data->ptr;
-      e.col[i].out_valid = c.validity ? (uint32_t *)c.validity->ptr : nullptr;
-      e.col[i].op = outs[i].op;
-      e.col[i].out_type = outs[i].out_type;
-      e.col[i].slot = outs[i].slot;
-      e.col[i].slot2 = outs[i].slot2;
-      e.col[i].xform = outs[i].xform;
+      if (outs[i].op == OUT_MOMENT) continue;
+      SB_REQUIRE(e.ncols < 2 * AGG_MAX_SLOTS, "too many aggregate output columns");
+      EmitCol &ec = e.col[e.ncols++];
+      ec.out = c.data->ptr;
+      ec.out_valid = c.validity ? (uint32_t *)c.validity->ptr : nullptr;
+      ec.op = outs[i].op;
+      ec.out_type = outs[i].out_type;
+      ec.slot = outs[i].slot;
+      ec.slot2 = outs[i].slot2;
+      ec.xform = outs[i].xform;
     }
     if (ngroups > 0) {
       agg_emit_kernel<<<(unsigned)((ngroups + 255) / 256), 256, 0, st>>>(e);
       SB_LAUNCH_CHECK();
     }
+    for (size_t j = 0; j < mom_out.size(); j++) {
+      const int first = plan->nkeys + mom_first_out[j];
+      for (int k = 0; k < (emit_buffers ? 3 : 1); k++) mom_out[j].out[k] = t->cols[first + k].data->ptr;
+      mom_out[j].out_valid = emit_buffers ? nullptr : (uint32_t *)t->cols[first].validity->ptr;
+    }
+    moments_run(a, mom_in, mom_out, final_mode, emit_buffers, slot_ids.as<int64_t>(), ngroups, st);
     // no host synchronisation: the table buffers stay valid until after the emit kernel in stream order
   } catch (...) {
     table_free(t);

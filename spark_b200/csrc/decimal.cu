@@ -15,6 +15,7 @@
 #include <vector>
 #include "decimal.cuh"
 #include "expr.cuh"
+#include "moments.cuh"
 
 namespace sb {
 
@@ -156,7 +157,7 @@ bool plan_has_decimal_sums(const sb_table *in, const sb_agg_plan *plan) {
     if (pos >= (int)in->cols.size()) return false;
     const bool dec = (sp.func == SB_AGG_SUM || sp.func == SB_AGG_AVG) && is_decimal(in->cols[pos].type);
     if (dec) return true;
-    pos += sp.func == SB_AGG_AVG ? 2 : 1;
+    pos += agg_buffer_width(sp.func);
   }
   return false;
 }
@@ -224,7 +225,7 @@ void hash_aggregate_decimals(const sb_table *in, const sb_agg_plan *plan, cudaSt
     int pos = plan->nkeys;
     for (int i = 0; i < plan->naggs; i++) {
       const sb_agg_spec &sp = plan->aggs[i];
-      const int nbuf = sp.func == SB_AGG_AVG ? 2 : 1;
+      const int nbuf = agg_buffer_width(sp.func);
       SB_REQUIRE(pos < (int)in->cols.size(), "Final aggregate expects buffer column %d but the input has %zu columns", pos, in->cols.size());
       const bool dec = (sp.func == SB_AGG_SUM || sp.func == SB_AGG_AVG) && is_decimal(in->cols[pos].type);
       info[i].first_spec = (int)specs.size();
@@ -287,12 +288,12 @@ void hash_aggregate_decimals(const sb_table *in, const sb_agg_plan *plan, cudaSt
   sb_table *t = table_new(g);
   try {
     for (int k = 0; k < plan->nkeys; k++) t->cols.push_back(column_share(res->cols[k]));
-    // output position of rewritten spec j inside `res`: every spec but a non-decimal AVG in a buffer-emitting mode yields one column
+    // output position of rewritten spec j inside `res`: one result column, or in a buffer-emitting mode the spec's buffer columns
     std::vector<int> spec_col(specs.size() + 1);
     int at = plan->nkeys;
     for (size_t j = 0; j < specs.size(); j++) {
       spec_col[j] = at;
-      at += (specs[j].func == SB_AGG_AVG && emit_buffers) ? 2 : 1;
+      at += emit_buffers ? agg_buffer_width(specs[j].func) : 1;
     }
     spec_col[specs.size()] = at;
     SB_REQUIRE(at == (int)res->cols.size(), "internal: aggregate result has %zu columns, expected %d", res->cols.size(), at);

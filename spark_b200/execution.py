@@ -254,10 +254,12 @@ class HashAggregateExec(SparkPlan):
                     dec = pos < len(schema.types) and schema.types[pos] in (capi.SB_DECIMAL64, capi.SB_DECIMAL128)
                 else:
                     dec = isinstance(fn.child, AttributeReference) and schema.types[schema.index(fn.child.name)] in (capi.SB_DECIMAL64, capi.SB_DECIMAL128)
-            pos += 2 if (fn.func == "avg" or (dec and fn.func == "sum")) else 1
+            moment = fn.func in ("var_pop", "var_samp", "stddev_pop", "stddev_samp")
+            pos += 2 if (fn.func == "avg" or (dec and fn.func == "sum")) else (3 if moment else 1)
             if self.mode in ("partial", "partial_merge"):
-                bufs = {"sum": [name + "#sum"], "avg": [name + "#sum", name + "#count"], "count": [name + "#count"],
-                        "count_star": [name + "#count"], "min": [name + "#val"], "max": [name + "#val"]}[fn.func]
+                bufs = [name + "#n", name + "#avg", name + "#m2"] if moment else {
+                    "sum": [name + "#sum"], "avg": [name + "#sum", name + "#count"], "count": [name + "#count"],
+                    "count_star": [name + "#count"], "min": [name + "#val"], "max": [name + "#val"]}[fn.func]
                 if dec and fn.func == "sum":
                     bufs = [name + "#sum", name + "#isEmpty"]
                 names += bufs
@@ -289,7 +291,9 @@ class HashAggregateExec(SparkPlan):
         specs = (capi.sb_agg_spec * max(1, len(self.aggregateExpressions)))()
         for i, (fn, _name) in enumerate(self.aggregateExpressions):
             specs[i].func = capi.SB_AGG[fn.func]
-            if self.mode != "final" and fn.child is not None:
+            if not getattr(fn, "null_on_divide_by_zero", True):
+                specs[i].flags = capi.SB_AGG_FLAG_NAN_ON_DIVIDE_BY_ZERO
+            if self.mode not in ("final", "partial_merge") and fn.child is not None:   # merge modes read buffers positionally
                 ce = CompiledExpr(fn.child, schema)
                 keep.append(ce)
                 specs[i].input = ce.c

@@ -782,6 +782,37 @@ class Max(AggregateFunction):
     func = "max"
 
 
+# ---- central moments (expressions/aggregate/CentralMomentAgg.scala:49-290) -------------------------------------------------
+class _CentralMomentAgg(AggregateFunction):
+    """Buffer (n, avg, m2), all doubles.  The input is cast to DOUBLE (ImplicitCastInputTypes); with
+    null_on_divide_by_zero=False (spark.sql.legacy.statisticalAggregate) the _samp forms of one row give NaN, not NULL."""
+
+    def __init__(self, child, null_on_divide_by_zero=True):
+        super().__init__(Cast(_wrap(child), "double"))
+        self.null_on_divide_by_zero = null_on_divide_by_zero
+
+
+class StddevSamp(_CentralMomentAgg):
+    """stddev_samp / stddev: sqrt(m2 / (n - 1))."""
+    func = "stddev_samp"
+
+
+class StddevPop(_CentralMomentAgg):
+    func = "stddev_pop"
+
+
+class VarianceSamp(_CentralMomentAgg):
+    """var_samp / variance: m2 / (n - 1)."""
+    func = "var_samp"
+
+
+class VariancePop(_CentralMomentAgg):
+    func = "var_pop"
+
+
+Stddev, Variance = StddevSamp, VarianceSamp
+
+
 class SortOrder:
     """SortOrder(child, direction, nullOrdering) (SortOrder.scala:63); default null ordering: ASC -> NULLS
     FIRST, DESC -> NULLS LAST."""
